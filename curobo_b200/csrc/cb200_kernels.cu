@@ -211,14 +211,14 @@ __device__ __forceinline__ float cspace_dof(const FusedArgs &a, const RobotView 
 //   phase A: q load + c-space cost, FK, spheres (+ padded copy), tool poses + tool-pose cost
 //   phase B: self collision, scene collision (discrete | swept + speed metric), J^T backward, row cost
 // ------------------------------------------------------------------------------------------------
-template <bool SPLINE>
+template <bool SPLINE, int W = 32>
 __device__ __forceinline__ void row_phase_a(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e,
                                             int b, int h, float &cs_cost, float &pose_c) {
   const cb200_rollout_cfg &cfg = a.cfg;
   const int D = rv.D, S = rv.S, L = rv.L;
   cs_cost = 0.0f;
   #pragma unroll 1
-  for (int d = lane; d < D; d += 32) {
+  for (int d = lane; d < D; d += W) {
     const bspline::State4 st = load_row_state<SPLINE>(a, e, b, h, d, D);
     es.qv[d] = st.p;
     float gp;
@@ -227,14 +227,14 @@ __device__ __forceinline__ void row_phase_a(const FusedArgs &a, const RobotView 
     cs_cost += c;
     if (a.cspace_cost) a.cspace_cost[(size_t)e * D + d] = c;
   }
-  __syncwarp();
-  warp_fk(rv, es, lane);
-  warp_spheres(rv, es, lane, a.robot_spheres ? reinterpret_cast<float4 *>(a.robot_spheres) + (size_t)e * S : nullptr,
-               row_sphere_cfg(a, b, S));
+  row_sync<W>();
+  warp_fk<W>(rv, es, lane);
+  warp_spheres<W>(rv, es, lane, a.robot_spheres ? reinterpret_cast<float4 *>(a.robot_spheres) + (size_t)e * S : nullptr,
+                  row_sphere_cfg(a, b, S));
   pose_c = 0.0f;
   const bool do_pose = (a.goal_position != nullptr);
   #pragma unroll 1
-  for (int t = lane; t < L; t += 32) {
+  for (int t = lane; t < L; t += W) {
     const float *T = es.cumul + 12 * rv.tool_map[t];
     const V3 p = mk3(T[3], T[7], T[11]);
     const Q4 qt = quat_from_transform(T);
@@ -272,7 +272,7 @@ __device__ __forceinline__ void row_phase_a(const FusedArgs &a, const RobotView 
       if (a.pose_goalset_idx) a.pose_goalset_idx[(size_t)e * L + t] = po.goal_idx;
     }
   }
-  __syncwarp();
+  row_sync<W>();
 }
 
 // phase B1: self collision + scene collision.  Leaves the scene sphere-gradients in es.gsph and returns the
@@ -282,7 +282,7 @@ struct RowB1 {
   int bi, bj, nnz;
 };
 
-template <bool SWEEP, int SCENE, bool CULL2 = true>
+template <bool SWEEP, int SCENE, bool CULL2 = true, int W = 32>
 __device__ __forceinline__ RowB1 row_phase_b1(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e,
                                               int b, const float4 *prev_sph, const float4 *next_sph) {
   const cb200_rollout_cfg &cfg = a.cfg;
@@ -290,12 +290,12 @@ __device__ __forceinline__ RowB1 row_phase_b1(const FusedArgs &a, const RobotVie
   RowB1 r{0.0f, 0.0f, 0.0f, 0, 0, 0};
   // ---- self collision (reads padded spheres in gsph)
   if (cfg.self_weight > 0.0f && rv.P > 0) {
-    r.fmax = (rv.n_lp > 0) ? warp_self_collision_tiles<true, CULL2>(rv, es, lane, r.bi, r.bj)
-                           : warp_self_collision_pairs(es.gsph, rv.pairs, rv.P, lane, r.bi, r.bj);
+    r.fmax = (rv.n_lp > 0) ? warp_self_collision_tiles<true, CULL2, W>(rv, es, lane, r.bi, r.bj)
+                           : warp_self_collision_pairs<W>(es.gsph, rv.pairs, rv.P, lane, r.bi, r.bj);
     r.self_c = (r.fmax > 0.0f) ? 0.5f * cfg.self_weight * r.fmax : 0.0f;
   }
   if (a.self_cost && lane == 0) a.self_cost[e] = r.self_c;
-  __syncwarp();
+  row_sync<W>();
   // ---- scene collision (lane per sphere) -> gsph = gradient
   const bool do_scene = SCENE != 0 && cfg.scene_weight > 0.0f;
   const int env = (a.env_query_idx != nullptr) ? __ldg(a.env_query_idx + b) : 0;
@@ -313,7 +313,7 @@ __device__ __forceinline__ RowB1 row_phase_b1(const FusedArgs &a, const RobotVie
     cull = !SWEEP && rv.n_lp > 0 && ncub <= 32;
     if (cull) {
 #pragma unroll 1
-      for (int ca = lane; ca < rv.n_cl; ca += 32) {
+      for (int ca = lane; ca < rv.n_cl; ca += W) {
         const float4 cb = rv.cl_bound_scene[ca];
         uint32_t mask = 0u;
         if (cb.w >= 0.0f) {
@@ -332,11 +332,11 @@ __device__ __forceinline__ RowB1 row_phase_b1(const FusedArgs &a, const RobotVie
         }
         es.cmask[ca] = mask;
       }
-      __syncwarp();
+      row_sync<W>();
     }
   }
 #pragma unroll 1
-  for (int s = lane; s < S; s += 32) {
+  for (int s = lane; s < S; s += W) {
     V3 g = mk3(0, 0, 0);
     float c = 0.0f;
     if (do_scene) {
@@ -390,13 +390,13 @@ __device__ __forceinline__ RowB1 row_phase_b1(const FusedArgs &a, const RobotVie
     r.scene_c += c;
     if (a.scene_cost) a.scene_cost[(size_t)e * S + s] = c;
   }
-  __syncwarp();
-  r.nnz = (int)__reduce_add_sync(kFull, (unsigned)r.nnz) + 2;  // + the two self-collision spheres
+  row_sync<W>();
+  r.nnz = (int)row_reduce<W, 0>((unsigned)r.nnz) + 2;  // + the two self-collision spheres
   return r;
 }
 
 // phase B2: add the self-collision gradient to the two spheres of the worst pair, J^T backward, row cost.
-template <bool SMALL = false>
+template <bool SMALL = false, int W = 32>
 __device__ __forceinline__ void row_phase_b2(const FusedArgs &a, const RobotView &rv, const EvalSmem &es,
                                              const unsigned char *smem_blob, int lane, int e, const RowB1 &r,
                                              float cs_cost, float pose_c) {
@@ -414,12 +414,12 @@ __device__ __forceinline__ void row_phase_b2(const FusedArgs &a, const RobotView
     es.gsph[r.bi] = gi;
     es.gsph[r.bj] = gj;
   }
-  __syncwarp();
+  row_sync<W>();
   float *gq = a.grad_q + (size_t)e * rv.D;
-  if (!warp_fk_backward_sparse<SMALL>(rv, es, lane, gq, r.nnz)) warp_fk_backward_cold(smem_blob, a.blob, es.cumul, lane, gq);
-  const float tot = warp_sum(cs_cost + pose_c + r.scene_c) + r.self_c;
+  if (!warp_fk_backward_sparse<SMALL, W>(rv, es, lane, gq, r.nnz)) warp_fk_backward_cold<W>(smem_blob, a.blob, es.cumul, lane, gq);
+  const float tot = warp_sum<W>(cs_cost + pose_c + r.scene_c) + r.self_c;
   if (lane == 0) a.cost[e] = tot;
-  __syncwarp();
+  row_sync<W>();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -433,68 +433,81 @@ __device__ __forceinline__ void row_phase_b2(const FusedArgs &a, const RobotView
 struct PhaseAOut {
   float cs_cost, pose_c;
 };
+template <int W>
 static __device__ __noinline__ PhaseAOut phase_a_ool(const FusedArgs *a, const unsigned char *smem, float *base, int lane,
                                                      int e, int b, int h) {
   const RobotView rv = make_robot_view(smem, a->blob);
   const EvalSmem es = carve_eval_smem(base, rv.nl, rv.D, rv.S, rv.L, rv.n_cl);
   PhaseAOut o;
-  row_phase_a<false>(*a, rv, es, lane, e, b, h, o.cs_cost, o.pose_c);
+  row_phase_a<false, W>(*a, rv, es, lane, e, b, h, o.cs_cost, o.pose_c);
   return o;
 }
-template <int SCENE>
+template <int SCENE, int W>
 static __device__ __noinline__ RowB1 phase_b1_ool(const FusedArgs *a, const unsigned char *smem, float *base, int lane, int e,
                                                   int b) {
   const RobotView rv = make_robot_view(smem, a->blob);
   const EvalSmem es = carve_eval_smem(base, rv.nl, rv.D, rv.S, rv.L, rv.n_cl);
-  return row_phase_b1<false, SCENE>(*a, rv, es, lane, e, b, nullptr, nullptr);
+  return row_phase_b1<false, SCENE, W == 32, W>(*a, rv, es, lane, e, b, nullptr, nullptr);
 }
+template <int W>
 static __device__ __noinline__ void phase_b2_ool(const FusedArgs *a, const unsigned char *smem, float *base, int lane, int e,
                                                  RowB1 r, float cs_cost, float pose_c) {
   const RobotView rv = make_robot_view(smem, a->blob);
   const EvalSmem es = carve_eval_smem(base, rv.nl, rv.D, rv.S, rv.L, rv.n_cl);
-  row_phase_b2(*a, rv, es, smem, lane, e, r, cs_cost, pose_c);
+  row_phase_b2<W == 16, W>(*a, rv, es, smem, lane, e, r, cs_cost, pose_c);
 }
 #endif  // CB200_OOL_PHASES
 
-template <int SCENE, bool SPLINE, int MINB = CB200_MINB>
+// ROWS = 2 (arm build only, robots of <= 16 links): two rows per warp, half h = lane >> 4 owns row 2 u + h of the warp's work
+// unit u, with the row helpers at width 16.  The halves run the same code on different rows and may diverge inside a row; they
+// meet again at the end of it, where the next unit is fetched.  A row's result does not depend on its partner.
+template <int SCENE, bool SPLINE, int MINB = CB200_MINB, int ROWS = 1>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB) rollout_fused_kernel(const __grid_constant__ FusedArgs a) {
+  static_assert(ROWS == 1 || (ROWS == 2 && MINB == 3 && !SPLINE), "paired rows: arm build only");
+  constexpr int W = 32 / ROWS;
   CB200_EXTERN_SHARED __align__(128) unsigned char smem[];
   __shared__ unsigned long long mbar;
   stage_blob_to_smem(smem, a.blob, (uint32_t)a.blob_smem_bytes, &mbar);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  float *base = reinterpret_cast<float *>(smem + a.blob_smem_bytes) + (size_t)warp * a.eval_floats;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & (W - 1), nwarps = blockDim.x >> 5;
+  const int half = ROWS == 1 ? 0 : (int)(threadIdx.x >> 4) & 1;
+  const bool leader = (threadIdx.x & 31) == 0;
+  float *base = reinterpret_cast<float *>(smem + a.blob_smem_bytes) + (size_t)(warp * ROWS + half) * a.eval_floats;
   const int N = a.B * a.H;
   const int stride = gridDim.x * nwarps;
-  // rows: the first one statically, the rest from the ticket counter when the caller provides one (rows differ in cost and
-  // 16,384 rows over 3,168 resident warps -- 132 SMs x 24 on an H100 -- is 5.2 rounds: with static striding the last round is partly empty)
-  int e = blockIdx.x * nwarps + warp;
-  while (e < N) {
-    int b = e, h = 0;
-    if (a.H != 1) {  // integer division is ~60 instructions: skip it for H == 1 (IK)
-      b = e / a.H;
-      h = e - b * a.H;
-    }
+  // work units (one row per warp, or one pair of rows): the first one statically, the rest from the ticket counter when the
+  // caller provides one (rows differ in cost and 16,384 rows over 3,168 resident warps -- 132 SMs x 24 on an H100 -- is 5.2
+  // rounds: with static striding the last round is partly empty)
+  int u = blockIdx.x * nwarps + warp;
+  while (u * ROWS < N) {
+    const int e = u * ROWS + half;
+    if (ROWS == 1 || e < N) {  // (odd N: the last unit's second half has no row)
+      int b = e, h = 0;
+      if (a.H != 1) {  // integer division is ~60 instructions: skip it for H == 1 (IK)
+        b = e / a.H;
+        h = e - b * a.H;
+      }
 #ifndef CB200_OOL_PHASES
-    const RobotView rv = make_robot_view(smem, a.blob);
-    const EvalSmem es = carve_eval_smem(base, rv.nl, rv.D, rv.S, rv.L, rv.n_cl);
-    float cs_cost = 0.0f, pose_c = 0.0f;
-    row_phase_a<SPLINE>(a, rv, es, lane, e, b, h, cs_cost, pose_c);
-    const RowB1 r = row_phase_b1<false, SCENE, MINB != 3>(a, rv, es, lane, e, b, nullptr, nullptr);
-    row_phase_b2<MINB == 3>(a, rv, es, smem, lane, e, r, cs_cost, pose_c);
+      const RobotView rv = make_robot_view(smem, a.blob);
+      const EvalSmem es = carve_eval_smem(base, rv.nl, rv.D, rv.S, rv.L, rv.n_cl);
+      float cs_cost = 0.0f, pose_c = 0.0f;
+      row_phase_a<SPLINE, W>(a, rv, es, lane, e, b, h, cs_cost, pose_c);
+      const RowB1 r = row_phase_b1<false, SCENE, MINB != 3, W>(a, rv, es, lane, e, b, nullptr, nullptr);
+      row_phase_b2<MINB == 3, W>(a, rv, es, smem, lane, e, r, cs_cost, pose_c);
 #else
-    const PhaseAOut pa = phase_a_ool(&a, smem, base, lane, e, b, h);
-    const RowB1 r = phase_b1_ool<SCENE>(&a, smem, base, lane, e, b);
-    phase_b2_ool(&a, smem, base, lane, e, r, pa.cs_cost, pa.pose_c);
+      const PhaseAOut pa = phase_a_ool<W>(&a, smem, base, lane, e, b, h);
+      const RowB1 r = phase_b1_ool<SCENE, W>(&a, smem, base, lane, e, b);
+      phase_b2_ool<W>(&a, smem, base, lane, e, r, pa.cs_cost, pa.pose_c);
 #endif
+    }
     if (a.work_counter != nullptr) {
       int nxt = 0;
-      if (lane == 0) nxt = stride + atomicAdd(a.work_counter, 1);
-      e = __shfl_sync(kFull, nxt, 0);
+      if (leader) nxt = stride + atomicAdd(a.work_counter, 1);
+      u = __shfl_sync(kFull, nxt, 0);
     } else {
-      e += stride;
+      u += stride;
     }
   }
-  if (a.work_counter != nullptr && lane == 0) {  // the last warp to leave re-arms the counter for the next launch
+  if (a.work_counter != nullptr && leader) {  // the last warp to leave re-arms the counter for the next launch
     __threadfence();
     if (atomicAdd(a.work_counter + 1, 1) == stride - 1) {
       a.work_counter[0] = 0;
@@ -3498,10 +3511,23 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
     CB200_LAUNCH(dk, (int)(grid_ll < 1 ? 1 : grid_ll), dpl.nw * 32, dpl.smem, (cudaStream_t)stream, a, dpl.R);
     return finish();
   }
+  // rows per warp: 2 for arms of <= 16 links (one link per lane of a half-warp in the sparse J^T) from 1.5 rows per resident warp
+  // slot of the arm build (MINB CTAs of kWarpsPerCta warps per SM) up; with fewer rows a warp per row is faster (Franka + cuboids,
+  // H100 SXM at 400 W: 0.0183 vs 0.0255 ms at 1.0 rows per slot, 0.0274 vs 0.0270 ms at 1.5, 0.0324 vs 0.0271 ms at 2.0).  Not
+  // against an ESDF: that build spills (140 B) and measured 2 % slower (franka_16384_esdf).  CB200_ARM_PAIRS = 0 / 1 forces one /
+  // two rows per warp.
+  int rows_per_warp = 1;
   if (variant == 0 && arm_regcap != 0 && (scene <= 1 || arm_esdf != 0) && h.nl <= 24 && h.S <= 128) {
-    kern = arm_table[scene];
-    variant = 5;
+    const char *ps = getenv("CB200_ARM_PAIRS");  // read per call: tests switch it inside one process
+    const int pairs_env = ps ? atoi(ps) : -1;
+    const bool pairs = h.nl <= 16 && (scene & 2) == 0 &&
+                       (pairs_env >= 0 ? pairs_env != 0 : 2LL * N >= 3LL * d.sm_count * 3 * kWarpsPerCta);
+    static KernelT const arm_pairs_table[2] = {rollout_fused_kernel<0, false, 3, 2>, rollout_fused_kernel<1, false, 3, 2>};
+    kern = pairs ? arm_pairs_table[scene] : arm_table[scene];
+    rows_per_warp = pairs ? 2 : 1;
+    variant = pairs ? 6 : 5;
   }
+  const int warp_floats = rows_per_warp * a.eval_floats;
   const int minb = scene;  // part of the plan-cache key
   // warps per CTA: the count that keeps the most warps resident per SM (shared memory is the limiter for
   // big robots); ties go to the larger CTA so the blob is staged fewer times.  Cached per (kernel, geometry).
@@ -3509,17 +3535,17 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
     long long key = -1;
     int nw = 0, per_sm = 0;
   };
-  static thread_local Plan plans[6][4];
+  static thread_local Plan plans[7][4];
   Plan &pl = plans[variant][scene];
   const size_t halo_bytes = traj ? (size_t)2 * h.S * sizeof(float4) : 0;
-  const long long key = ((long long)h.smem_bytes << 32) ^ ((long long)a.eval_floats << 8) ^ (long long)minb ^
+  const long long key = ((long long)h.smem_bytes << 32) ^ ((long long)warp_floats << 8) ^ (long long)minb ^
                         (traj ? ((long long)io->horizon << 40) : 0) ^ ((long long)(d.ordinal + 1) << 56);
   if (key != pl.key) {
     cudaFuncAttributes fa;
     cudaError_t e0 = cudaFuncGetAttributes(&fa, kern);
     if (e0 != cudaSuccess) return ret(e0);
     const size_t limit = (size_t)d.max_smem - fa.sharedSizeBytes;  // opt-in limit covers static + dynamic
-    const size_t max_need = (size_t)h.smem_bytes + halo_bytes + (size_t)kWarpsPerCta * a.eval_floats * sizeof(float);
+    const size_t max_need = (size_t)h.smem_bytes + halo_bytes + (size_t)kWarpsPerCta * warp_floats * sizeof(float);
     const size_t cap = std::min(max_need, limit);
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cap);
     if (e != cudaSuccess) return ret(e);
@@ -3531,7 +3557,7 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
     }();
     for (int nw = kWarpsPerCta; nw >= 1; --nw) {
       if (force_nw > 0 && nw != force_nw) continue;
-      const size_t need = (size_t)h.smem_bytes + halo_bytes + (size_t)nw * a.eval_floats * sizeof(float);
+      const size_t need = (size_t)h.smem_bytes + halo_bytes + (size_t)nw * warp_floats * sizeof(float);
       if (need > limit) continue;
       int per_sm = 0;
       if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, nw * 32, need) != cudaSuccess) continue;
@@ -3557,13 +3583,14 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
     a.work_counter = !(qs && atoi(qs) == 0) ? io->work_counter : nullptr;
     if (traj && (long long)io->batch_size * ((io->horizon + nw - 1) / nw) > 0x3fffffffLL) a.work_counter = nullptr;  // int tickets
   }
-  const size_t smem = (size_t)h.smem_bytes + halo_bytes + (size_t)nw * a.eval_floats * sizeof(float);
+  const size_t smem = (size_t)h.smem_bytes + halo_bytes + (size_t)nw * warp_floats * sizeof(float);
   long long grid_ll = (long long)d.sm_count * pl.per_sm;
-  const long long need_ctas = traj ? (long long)io->batch_size * ((io->horizon + nw - 1) / nw) : (N + nw - 1) / nw;
+  const long long units = (N + rows_per_warp - 1) / rows_per_warp;  // rows, or pairs of rows
+  const long long need_ctas = traj ? (long long)io->batch_size * ((io->horizon + nw - 1) / nw) : (units + nw - 1) / nw;
   if (grid_ll > need_ctas) grid_ll = need_ctas;
   const int grid = (int)(grid_ll < 1 ? 1 : grid_ll);
-  if (need_ctas <= grid_ll) a.work_counter = nullptr;  // every row / tile has its own warp / CTA: nothing to hand out
-  g_last_variant = traj ? CB200_VARIANT_TRAJ : (variant == 5 ? CB200_VARIANT_ARM : CB200_VARIANT_STANDARD);
+  if (need_ctas <= grid_ll) a.work_counter = nullptr;  // every row / pair / tile has its own warp / CTA: nothing to hand out
+  g_last_variant = traj ? CB200_VARIANT_TRAJ : (variant >= 5 ? CB200_VARIANT_ARM : CB200_VARIANT_STANDARD);
   CB200_LAUNCH(kern, grid, nw * 32, smem, (cudaStream_t)stream, a);
   return finish();
 }

@@ -144,9 +144,104 @@ __device__ __forceinline__ EvalSmem carve_big_smem(float *base, int nl, int D, i
   return e;
 }
 
+// Lanes of one row.  W = 32: the whole warp.  W = 16 (paired arm build): half h = lane >> 4 of the warp owns a row of its own,
+// and the two halves may diverge, so every collective of a row names the row's lanes only.  In the helpers below `lane` is the
+// lane within the row (0 .. W-1) and ballots come back in row-local bits.  W = 32 spells exactly the full-warp intrinsics.
+template <int W>
+__device__ __forceinline__ unsigned row_mask() {
+  static_assert(W == 32 || W == 16, "a row is a warp or a half-warp");
+  return W == 32 ? kFull : 0xffffu << (threadIdx.x & 16u);
+}
+#ifdef CB200_SIMT_EMULATION
+// Host emulation build (tests/simt): there a warp collective is a meeting of all 32 lane threads, whatever its mask, while the
+// two halves of a paired warp may be on different paths.  A half-warp's collectives therefore meet on a named barrier of their
+// own (id = the half's index in the CTA: 16 ids for the <= 8-warp CTAs of the paired build), values passing through a CTA-wide
+// slot array: publish, meet, read the half's 16 slots, meet again so the slots can be reused.
+template <class T, class F>
+inline T half_exchange(T v, F pick) {
+  static unsigned long long slot[16 * 16];
+  const int t = threadIdx.x;
+  unsigned long long bits = 0;
+  std::memcpy(&bits, &v, sizeof(T));
+  slot[t] = bits;
+  simt::named_barrier(t >> 4, 16);
+  const unsigned long long got = pick(slot + (t & ~15));
+  simt::named_barrier(t >> 4, 16);
+  T r;
+  std::memcpy(&r, &got, sizeof(T));
+  return r;
+}
+#endif
+template <int W>
+__device__ __forceinline__ void row_sync() {
+  if (W == 32) {
+    __syncwarp();
+  } else {
+#ifdef CB200_SIMT_EMULATION
+    simt::named_barrier(threadIdx.x >> 4, 16);
+#else
+    __syncwarp(row_mask<W>());
+#endif
+  }
+}
+template <int W>
+__device__ __forceinline__ unsigned row_ballot(bool p) {
+  if (W == 32) return __ballot_sync(kFull, p);
+#ifdef CB200_SIMT_EMULATION
+  return half_exchange((unsigned)p, [](const unsigned long long *s) {
+    unsigned long long m = 0;
+    for (int i = 0; i < 16; ++i) m |= (s[i] & 1ull) << i;
+    return m;
+  });
+#else
+  const unsigned m = row_mask<W>();
+  return (__ballot_sync(m, p) & m) >> (threadIdx.x & 16u);
+#endif
+}
+// value of row lane `src`
+template <int W>
+__device__ __forceinline__ uint32_t row_shfl(uint32_t v, int src) {
+  if (W == 32) return __shfl_sync(kFull, v, src);
+#ifdef CB200_SIMT_EMULATION
+  return half_exchange(v, [src](const unsigned long long *s) { return s[src & 15]; });
+#else
+  return __shfl_sync(row_mask<W>(), v, src, W);
+#endif
+}
+// value of row lane `lane ^ o` (o < W)
+template <int W, class T>
+__device__ __forceinline__ T row_shfl_xor(T v, int o) {
+  if (W == 32) return __shfl_xor_sync(kFull, v, o);
+#ifdef CB200_SIMT_EMULATION
+  const int me = threadIdx.x & 15;
+  return half_exchange(v, [me, o](const unsigned long long *s) { return s[me ^ o]; });
+#else
+  return __shfl_xor_sync(row_mask<W>(), v, o);
+#endif
+}
+// REDUX over the row's lanes: OP 0 = add, 1 = min, 2 = max
+template <int W, int OP>
+__device__ __forceinline__ unsigned row_reduce(unsigned v) {
+  if (W == 32) return OP == 0 ? __reduce_add_sync(kFull, v) : OP == 1 ? __reduce_min_sync(kFull, v) : __reduce_max_sync(kFull, v);
+#ifdef CB200_SIMT_EMULATION
+  return half_exchange(v, [](const unsigned long long *s) {
+    unsigned r = (unsigned)s[0];
+    for (int i = 1; i < 16; ++i) {
+      const unsigned x = (unsigned)s[i];
+      r = OP == 0 ? r + x : OP == 1 ? (x < r ? x : r) : (x > r ? x : r);
+    }
+    return (unsigned long long)r;
+  });
+#else
+  const unsigned m = row_mask<W>();
+  return OP == 0 ? __reduce_add_sync(m, v) : OP == 1 ? __reduce_min_sync(m, v) : __reduce_max_sync(m, v);
+#endif
+}
+
+template <int W = 32>
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
+  for (int o = W / 2; o > 0; o >>= 1) v += row_shfl_xor<W>(v, o);
   return v;
 }
 
@@ -155,29 +250,34 @@ __device__ __forceinline__ float warp_sum(float v) {
 // (12 lanes per link, two links per step).  cumul[l] = cumul[parent[l]] * local[l].
 // Reference semantics: kinematics_forward_helper.cuh:316-512.
 // ----------------------------------------------------------------------------------------------
+template <int W = 32>
 __device__ __forceinline__ void warp_fk_compose(const RobotView &rv, const EvalSmem &es, int lane);
+template <int W = 32>
 __device__ __forceinline__ void warp_fk(const RobotView &rv, const EvalSmem &es, int lane) {
   // local transforms go to a scratch buffer (the not-yet-written world-sphere area) when it is large enough,
   // so a compose step needs one warp barrier instead of two; otherwise they are composed in place.
   const bool scratch = rv.S * 4 >= rv.nl * 12;
   float *loc = scratch ? reinterpret_cast<float *>(es.sph) : es.cumul;
   #pragma unroll 1
-  for (int l = lane; l < rv.nl; l += 32) {
+  for (int l = lane; l < rv.nl; l += W) {
     int jt = rv.joint_type[l];
     float th = 0.0f;
     if (jt >= 0) th = rv.joff[2 * l] * es.qv[rv.joint_map[l]] + rv.joff[2 * l + 1];
     local_link_transform(rv.fixed + 12 * l, jt, th, (l == 0 ? es.cumul : loc) + 12 * l);
   }
-  __syncwarp();
-  warp_fk_compose(rv, es, lane);
+  row_sync<W>();
+  warp_fk_compose<W>(rv, es, lane);
 }
 
 // second half of warp_fk: the level-scheduled compose (the local transforms are in place; see warp_fk)
+template <int W>
 __device__ __forceinline__ void warp_fk_compose(const RobotView &rv, const EvalSmem &es, int lane) {
   const bool scratch = rv.S * 4 >= rv.nl * 12;
   const float *loc = scratch ? reinterpret_cast<const float *>(es.sph) : es.cumul;
-  // compose: 12 lanes per link, two links (same depth level) per step; the schedule holds byte offsets
-  const int sub = lane >> 4, k = lane & 15;
+  // compose: 12 lanes per link, two links (same depth level) per step; the schedule holds byte offsets.  A whole warp does the
+  // two links at once (half-warp per link); a half-warp row does slot 0, then slot 1 -- the schedule is the robot's, so both
+  // rows of a warp take the same branches here.
+  const int half = lane >> 4, k = lane & 15;
   const bool lane_ok = k < 12;
   const uint32_t row_off = (uint32_t)(k >> 2) * 16u, col_off = (uint32_t)(k & 3) * 4u, k_off = (uint32_t)k * 4u;
   const float cw = ((k & 3) == 3) ? 1.0f : 0.0f;
@@ -185,18 +285,23 @@ __device__ __forceinline__ void warp_fk_compose(const RobotView &rv, const EvalS
   const unsigned char *locb = reinterpret_cast<const unsigned char *>(loc);
 #pragma unroll 1
   for (int st = 0; st < rv.n_fk_steps; ++st) {
-    const uint32_t w = rv.fk_sched[2 * st + sub];
-    const uint32_t l_off = w & 0xffffu, p_off = w >> 16;
-    const bool act = lane_ok && (l_off != 0xffffu);
-    float out = 0.0f;
-    if (act) {
-      const float4 pr = *reinterpret_cast<const float4 *>(cumb + p_off + row_off);
-      const float *Lm = reinterpret_cast<const float *>(locb + l_off + col_off);
-      out = pr.x * Lm[0] + pr.y * Lm[4] + pr.z * Lm[8] + cw * pr.w;
+#pragma unroll
+    for (int pass = 0; pass < 32 / W; ++pass) {
+      const int sub = W == 32 ? half : pass;
+      const uint32_t w = rv.fk_sched[2 * st + sub];
+      const uint32_t l_off = w & 0xffffu, p_off = w >> 16;
+      if (W == 16 && l_off == 0xffffu) continue;  // empty slot (same for every row)
+      const bool act = lane_ok && (l_off != 0xffffu);
+      float out = 0.0f;
+      if (act) {
+        const float4 pr = *reinterpret_cast<const float4 *>(cumb + p_off + row_off);
+        const float *Lm = reinterpret_cast<const float *>(locb + l_off + col_off);
+        out = pr.x * Lm[0] + pr.y * Lm[4] + pr.z * Lm[8] + cw * pr.w;
+      }
+      if (!scratch) row_sync<W>();
+      if (act) *reinterpret_cast<float *>(cumb + l_off + k_off) = out;
+      row_sync<W>();
     }
-    if (!scratch) __syncwarp();
-    if (act) *reinterpret_cast<float *>(cumb + l_off + k_off) = out;
-    __syncwarp();
   }
 }
 
@@ -204,10 +309,11 @@ __device__ __forceinline__ void warp_fk_compose(const RobotView &rv, const EvalS
 // Reference: kinematics_forward_helper.cuh:218-254, kinematics_util.cuh:39-49.
 // `cfg_spheres` != nullptr: the row's link-sphere configuration in global memory (num_envs > 1,
 // kinematics_forward_helper.cuh:232-233) instead of the blob's set.
+template <int W = 32>
 __device__ __forceinline__ void warp_spheres(const RobotView &rv, const EvalSmem &es, int lane, float4 *out_global,
                                              const float4 *cfg_spheres = nullptr) {
   #pragma unroll 1
-  for (int s = lane; s < rv.S; s += 32) {
+  for (int s = lane; s < rv.S; s += W) {
     const float *T = es.cumul + 12 * rv.sph_link[s];
     const float4 p = cfg_spheres != nullptr ? __ldg(cfg_spheres + s) : rv.spheres[s];
     const float4 r0 = *reinterpret_cast<const float4 *>(T), r1 = *reinterpret_cast<const float4 *>(T + 4),
@@ -232,12 +338,13 @@ __device__ __forceinline__ void warp_spheres(const RobotView &rv, const EvalSmem
 // Reference: self_collision_helper.cuh:61-71,227-277; collision_pair.cuh:55-57.
 // Returns f_max (0 if none) and the pair (i,j) to every lane.
 // ----------------------------------------------------------------------------------------------
+template <int W = 32>
 __device__ __forceinline__ float warp_self_collision_pairs(const float4 *psph, const uint32_t *pairs, int P, int lane,
                                                            int &bi, int &bj) {
   float best = 0.0f;
   uint32_t best_p = 0xffffffffu;
   #pragma unroll 1
-  for (int p = lane; p < P; p += 32) {
+  for (int p = lane; p < P; p += W) {
     const uint32_t pr = __ldg(pairs + p);
     const float4 a = psph[pr & 0xffffu], b = psph[pr >> 16];
     const float rs = a.w + b.w;
@@ -250,9 +357,9 @@ __device__ __forceinline__ float warp_self_collision_pairs(const float4 *psph, c
     }
   }
   // positive floats order like their bit patterns
-  const uint32_t fb = __reduce_max_sync(kFull, __float_as_uint(best));
+  const uint32_t fb = row_reduce<W, 2>(__float_as_uint(best));
   const uint32_t cand = (__float_as_uint(best) == fb && best > 0.0f) ? best_p : 0xffffffffu;
-  const uint32_t win = __reduce_min_sync(kFull, cand);
+  const uint32_t win = row_reduce<W, 1>(cand);
   bi = bj = 0;
   if (win == 0xffffffffu) return 0.0f;
   const uint32_t pr = __ldg(pairs + win);
@@ -284,20 +391,21 @@ __device__ __forceinline__ float4 padded_sphere(const RobotView &rv, const EvalS
 // key_out: the warp's reduced arg-max key (f bits | ~i | ~j), 0 when nothing is positive.
 // CULL2 = false (arm build of the IK kernel: links of <= ~10 spheres): blocks are scanned whole -- the second-level cull's code is
 // 1.6 KB of the row's instruction footprint, which is what that kernel is short of.
-template <bool PADDED_COPY = true, bool CULL2 = true>
+template <bool PADDED_COPY = true, bool CULL2 = true, int W = 32>
 __device__ __forceinline__ float warp_self_collision_tiles(const RobotView &rv, const EvalSmem &es, int lane, int &bi,
-                                                           int &bj, int base0 = 0, int stride = 32,
+                                                           int &bj, int base0 = 0, int stride = W,
                                                            unsigned char *idx_scratch = nullptr,
                                                            unsigned long long *key_out = nullptr, bool fill_bounds = true) {
+  static_assert(W == 32 || !CULL2, "the second-level cull is written for whole-warp rows");
   if (fill_bounds) {
     #pragma unroll 1
-    for (int a = lane; a < rv.n_cl; a += 32) {
+    for (int a = lane; a < rv.n_cl; a += W) {
       const float4 c = rv.cl_bound[a];
       const float *T = es.cumul + 12 * rv.cl_link[a];
       es.bc[a] = make_float4(T[0] * c.x + T[1] * c.y + T[2] * c.z + T[3], T[4] * c.x + T[5] * c.y + T[6] * c.z + T[7],
                              T[8] * c.x + T[9] * c.y + T[10] * c.z + T[11], c.w);
     }
-    __syncwarp();
+    row_sync<W>();
   }
   unsigned long long key = 0ull;  // f bits | ~i | ~j : max = largest f, then smallest i, then smallest j
   #pragma unroll 1
@@ -310,11 +418,11 @@ __device__ __forceinline__ float warp_self_collision_tiles(const RobotView &rv, 
       const float dx = A.x - B.x, dy = A.y - B.y, dz = A.z - B.z, rs = A.w + B.w;
       hit = (A.w >= 0.0f) && (B.w >= 0.0f) && (dx * dx + dy * dy + dz * dz < rs * rs);
     }
-    unsigned m = __ballot_sync(kFull, hit);
+    unsigned m = row_ballot<W>(hit);
     while (m) {
       const int src = __ffs(m) - 1;
       m &= m - 1;
-      const uint32_t q = __shfl_sync(kFull, pr, src);
+      const uint32_t q = row_shfl<W>(pr, src);
       const int a = q & 0xffffu, b = q >> 16;
       const int sa = rv.cl_start[a], na = rv.cl_start[a + 1] - sa;
       const int sb = rv.cl_start[b], nb = rv.cl_start[b + 1] - sb;
@@ -364,7 +472,7 @@ __device__ __forceinline__ float warp_self_collision_tiles(const RobotView &rv, 
       }
       const float inv_nb = 1.0f / (float)nb;
       #pragma unroll 1
-      for (int t = lane; t < na * nb; t += 32) {
+      for (int t = lane; t < na * nb; t += W) {
         const int io = (int)(((float)t + 0.5f) * inv_nb);
         const int i = sa + io, j = sb + (t - io * nb);
         const float4 x = padded_sphere<PADDED_COPY>(rv, es, i), y = padded_sphere<PADDED_COPY>(rv, es, j);
@@ -380,8 +488,8 @@ __device__ __forceinline__ float warp_self_collision_tiles(const RobotView &rv, 
     }
   }
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const unsigned long long other = __shfl_xor_sync(kFull, key, o);
+  for (int o = W / 2; o > 0; o >>= 1) {
+    const unsigned long long other = row_shfl_xor<W>(key, o);
     key = other > key ? other : key;
   }
   if (key_out != nullptr) *key_out = key;
@@ -401,10 +509,12 @@ __device__ __forceinline__ float warp_self_collision_tiles(const RobotView &rv, 
 // kinematics_joint_util.cuh:12-67): g.(a x (p-o_j)) = a.((p-o_j) x g).
 // gq_out[d] = gqv[d] + sum over links driven by joint d.
 // ----------------------------------------------------------------------------------------------
+template <int W = 32>
 __device__ __forceinline__ void warp_fk_upsweep(const RobotView &rv, const EvalSmem &es, int lane, float *gq_out);
+template <int W = 32>
 __device__ __forceinline__ void warp_fk_backward(const RobotView &rv, const EvalSmem &es, int lane, float *gq_out) {
   #pragma unroll 1
-  for (int k = lane; k < rv.nl; k += 32) {
+  for (int k = lane; k < rv.nl; k += W) {
     const float *Tk = es.cumul + 12 * k;
     const V3 o = mk3(Tk[3], Tk[7], Tk[11]);
     V3 F = mk3(0, 0, 0), T = mk3(0, 0, 0);
@@ -431,14 +541,15 @@ __device__ __forceinline__ void warp_fk_backward(const RobotView &rv, const Eval
     ft[5] = T.y;
     ft[6] = T.z;
   }
-  __syncwarp();
-  warp_fk_upsweep(rv, es, lane, gq_out);
+  row_sync<W>();
+  warp_fk_upsweep<W>(rv, es, lane, gq_out);
 }
 
 // second half of the J^T backward: per-link (F, T) accumulators in es.ft -> joint gradients
+template <int W>
 __device__ __forceinline__ void warp_fk_upsweep(const RobotView &rv, const EvalSmem &es, int lane, float *gq_out) {
   #pragma unroll 1
-  for (int j = lane; j < rv.nl; j += 32) {
+  for (int j = lane; j < rv.nl; j += W) {
     const int jt = rv.joint_type[j];
     float res = 0.0f;
     if (jt >= 0) {
@@ -461,8 +572,8 @@ __device__ __forceinline__ void warp_fk_upsweep(const RobotView &rv, const EvalS
     }
     es.contrib[j] = res;
   }
-  __syncwarp();
-  for (int d = lane; d < rv.D; d += 32) {
+  row_sync<W>();
+  for (int d = lane; d < rv.D; d += W) {
     float g = es.gqv[d];
     for (int i = rv.jl_off[d]; i < rv.jl_off[d + 1]; ++i) g += es.contrib[rv.jl_idx[i]];
     gq_out[d] = g;
@@ -471,11 +582,12 @@ __device__ __forceinline__ void warp_fk_upsweep(const RobotView &rv, const EvalS
 
 // Dense fallback, out of line: rarely taken, and inlining it would only bloat the instruction footprint of the
 // hot path.  Views are rebuilt from raw pointers so that the caller's RobotView/EvalSmem stay in registers.
+template <int W = 32>
 static __device__ __noinline__ void warp_fk_backward_cold(const unsigned char *smem_blob, const unsigned char *gmem_blob,
                                                           float *eval_base, int lane, float *gq_out) {
   const RobotView rv = make_robot_view(smem_blob, gmem_blob);
   const EvalSmem es = carve_eval_smem(eval_base, rv.nl, rv.D, rv.S, rv.L, rv.n_cl);
-  warp_fk_backward(rv, es, lane, gq_out);
+  warp_fk_backward<W>(rv, es, lane, gq_out);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -489,9 +601,11 @@ static __device__ __noinline__ void warp_fk_backward_cold(const unsigned char *s
 // SMALL = true (arm build: <= 24 links, so one link per lane, and <= 128 spheres): the second link slot is compiled out and the
 // tool frames ride through the same broadcast loop as the spheres (entries S .. S + L - 1) -- one copy of the accumulate code
 // instead of two; the row's instruction footprint is what that kernel is short of.
-template <bool SMALL = false>
+// W = 16 (half-warp rows): SMALL only, and the robot has <= 16 links.
+template <bool SMALL = false, int W = 32>
 __device__ __forceinline__ bool warp_fk_backward_sparse(const RobotView &rv, const EvalSmem &es, int lane, float *gq_out,
                                                         int nnz) {
+  static_assert(W == 32 || SMALL, "half-warp rows take the one-link-per-lane form");
   if (nnz > 2 * rv.nl) return false;  // nnz = spheres with a non-zero gradient (counted by the caller)
   if (SMALL) {
     float sc = 0.0f;
@@ -510,7 +624,7 @@ __device__ __forceinline__ bool warp_fk_backward_sparse(const RobotView &rv, con
     float acc = 0.0f;
     const int n_entries = rv.S + rv.L;
 #pragma unroll 1
-    for (int base = 0; base < n_entries; base += 32) {
+    for (int base = 0; base < n_entries; base += W) {
       const int s = base + lane;
       bool nz = false;
       if (s < rv.S) {
@@ -520,7 +634,7 @@ __device__ __forceinline__ bool warp_fk_backward_sparse(const RobotView &rv, con
         const float *pg = es.pose_g + 8 * (s - rv.S);
         nz = pg[0] != 0.0f || pg[1] != 0.0f || pg[2] != 0.0f || pg[4] != 0.0f || pg[5] != 0.0f || pg[6] != 0.0f;
       }
-      unsigned m = __ballot_sync(kFull, nz);
+      unsigned m = row_ballot<W>(nz);
       while (m) {
         const int ss = base + __ffs(m) - 1;
         m &= m - 1;
@@ -544,8 +658,8 @@ __device__ __forceinline__ bool warp_fk_backward_sparse(const RobotView &rv, con
       }
     }
     if (lane < rv.nl) es.contrib[lane] = acc;
-    __syncwarp();
-    for (int d = lane; d < rv.D; d += 32) {
+    row_sync<W>();
+    for (int d = lane; d < rv.D; d += W) {
       float g = es.gqv[d];
       for (int i = rv.jl_off[d]; i < rv.jl_off[d + 1]; ++i) g += es.contrib[rv.jl_idx[i]];
       gq_out[d] = g;

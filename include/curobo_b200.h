@@ -38,7 +38,7 @@ const char *cb200_error_string(int err);
    choice is made by the launcher from the robot, the scene content and the row count -- see DESIGN.md "Row scheduling"). */
 #define CB200_VARIANT_NONE 0
 #define CB200_VARIANT_STANDARD 1 /* rollout_fused_kernel: one warp per row */
-#define CB200_VARIANT_ARM 2      /* ... its 80-register build for arms against cuboids */
+#define CB200_VARIANT_ARM 2      /* ... its 80-register build for arms (one row per warp, or two: one per half-warp) */
 #define CB200_VARIANT_BIG 4      /* rollout_fused_big_kernel: humanoids / ESDF scenes, gradient list */
 #define CB200_VARIANT_TEAM2 5    /* rollout_fused_team_kernel: two warps per row */
 #define CB200_VARIANT_TEAM4 6    /* ... four warps per row */
