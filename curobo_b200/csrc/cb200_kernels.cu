@@ -77,6 +77,9 @@ struct FusedArgs {
   int32_t n_sphere_cfgs;
   // big-robot kernel: row ticket counter [2] (zero between launches; null = static striding)
   int32_t *work_counter;
+  // mesh obstacles (read by the SCENE & 4 builds only).  Last member, so the parameter offsets of the members above -- and the
+  // code of the builds without meshes -- do not depend on it.
+  MeshSet meshes;
 };
 
 // link-frame sphere set of seed b: the blob's (shared memory) unless the caller passed several configurations
@@ -282,6 +285,20 @@ struct RowB1 {
   int bi, bj, nnz;
 };
 
+// Mesh terms of one sphere (the SCENE & 4 builds): weighted world-frame gradient in xyz, weighted cost in w.  The caller adds them
+// to the cuboid + ESDF sum: the order of the per-operator composition, where one launch writes the cuboid + ESDF terms and the
+// mesh launch adds to them (cb200_sphere_mesh_collision with accumulate = 1).  Inlined: an out-of-line call spilled more than the
+// inlined traversal in every family (the registers live across the call are saved around it; DESIGN.md section 4).
+__device__ __forceinline__ float4 mesh_terms(const MeshSet *ms, float eta, float w, V3 c, float r, int env, bool sweep, bool has_prev,
+                                          V3 prev, bool has_next, V3 next) {
+  const CuboidSet no_cuboids{};
+  const VoxelSet no_voxels{};
+  V3 g = mk3(0, 0, 0);
+  const float cost = sweep ? sphere_scene_swept<4>(c, r, eta, w, has_prev, prev, has_next, next, no_cuboids, no_voxels, env, g, ms)
+                           : sphere_scene_discrete<4>(c, r, eta, w, no_cuboids, no_voxels, env, g, ms);
+  return make_float4(g.x, g.y, g.z, cost);
+}
+
 template <bool SWEEP, int SCENE, bool CULL2 = true, int W = 32>
 __device__ __forceinline__ RowB1 row_phase_b1(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e,
                                               int b, const float4 *prev_sph, const float4 *next_sph) {
@@ -304,9 +321,10 @@ __device__ __forceinline__ RowB1 row_phase_b1(const FusedArgs &a, const RobotVie
                         : 0.0f;
   // cuboid broad phase (discrete mode): a box SDF is 1-Lipschitz, so sdf(link bound centre) >= R_link + eta
   // means no sphere of the link has pen = r + eta - sdf > 0 against that cuboid -> skipping it is exact.
+  // (The mesh build, SCENE = 7, runs with or without cuboids and ESDF grids: it checks at run time which sets are present.)
   int ce = 0, ncub = 0;
   bool cull = false;
-  if ((SCENE & 1) && do_scene) {
+  if ((SCENE & 1) && do_scene && (!(SCENE & 4) || a.cuboids.inv_pose != nullptr)) {
     ce = env < a.cuboids.num_envs ? env : 0;
     ncub = a.cuboids.count[ce];
     if (ncub > a.cuboids.max_n) ncub = a.cuboids.max_n;
@@ -369,6 +387,11 @@ __device__ __forceinline__ RowB1 row_phase_b1(const FusedArgs &a, const RobotVie
             const CuboidSet none{};
             c += sphere_scene_discrete<2>(cen, sp.w, cfg.scene_activation, cfg.scene_weight, none, a.voxels, env, g);
           }
+          if (SCENE & 4) {
+            const float4 m = mesh_terms(&a.meshes, cfg.scene_activation, cfg.scene_weight, cen, sp.w, env, false, false, cen, false, cen);
+            c += m.w;
+            g = g + mk3(m.x, m.y, m.z);
+          }
         }
       } else {
         V3 pv = cen, nx = cen;
@@ -380,8 +403,14 @@ __device__ __forceinline__ RowB1 row_phase_b1(const FusedArgs &a, const RobotVie
           const float4 t = next_sph[s];
           nx = mk3(t.x, t.y, t.z);
         }
-        c = sphere_scene_swept<SCENE>(cen, sp.w, cfg.scene_activation, cfg.scene_weight, prev_sph != nullptr, pv,
-                                      next_sph != nullptr, nx, a.cuboids, a.voxels, env, g);
+        c = sphere_scene_swept<SCENE & 3>(cen, sp.w, cfg.scene_activation, cfg.scene_weight, prev_sph != nullptr, pv,
+                                          next_sph != nullptr, nx, a.cuboids, a.voxels, env, g);
+        if (SCENE & 4) {
+          const float4 m = mesh_terms(&a.meshes, cfg.scene_activation, cfg.scene_weight, cen, sp.w, env, true, prev_sph != nullptr,
+                                      pv, next_sph != nullptr, nx);
+          c += m.w;
+          g = g + mk3(m.x, m.y, m.z);
+        }
         if (cfg.use_speed_metric && prev_sph != nullptr && next_sph != nullptr) speed_metric(pv, cen, nx, sdt, c, g);
       }
     }
@@ -547,7 +576,7 @@ __device__ __forceinline__ RowB1 row_phase_b1_list(const FusedArgs &a, const Rob
   const int env = (a.env_query_idx != nullptr) ? __ldg(a.env_query_idx + b) : 0;
   int ce = 0, ncub = 0;
   bool cull = false;
-  if ((SCENE & 1) && do_scene) {  // cuboid broad phase, as in row_phase_b1
+  if ((SCENE & 1) && do_scene && (!(SCENE & 4) || a.cuboids.inv_pose != nullptr)) {  // cuboid broad phase, as in row_phase_b1
     ce = env < a.cuboids.num_envs ? env : 0;
     ncub = a.cuboids.count[ce];
     if (ncub > a.cuboids.max_n) ncub = a.cuboids.max_n;
@@ -611,6 +640,11 @@ __device__ __forceinline__ RowB1 row_phase_b1_list(const FusedArgs &a, const Rob
         if (SCENE & 2) {
           const CuboidSet none{};
           c += sphere_scene_discrete<2>(cen, sp.w, cfg.scene_activation, cfg.scene_weight, none, a.voxels, env, g);
+        }
+        if (SCENE & 4) {
+          const float4 m = mesh_terms(&a.meshes, cfg.scene_activation, cfg.scene_weight, cen, sp.w, env, false, false, cen, false, cen);
+          c += m.w;
+          g = g + mk3(m.x, m.y, m.z);
         }
       }
     }
@@ -3180,6 +3214,17 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
   a.phase_sync = phase_sync_env;
   const bool expand = sp != nullptr && sp->out_position != nullptr && sp->out_velocity != nullptr &&
                       sp->out_acceleration != nullptr && sp->out_jerk != nullptr && sp->out_dt != nullptr;
+  // mesh obstacles: scene bit 2.  The in-kernel spline schedule and the fused-dynamics kernel have no mesh build; they refuse mesh
+  // scenes rather than drop the meshes (the expanded schedule and the host-composed dynamics cost support them).
+  const bool mesh = cfg->scene_weight > 0.0f && io->meshes != nullptr && io->meshes->inv_pose != nullptr;
+  if (mesh) {
+    const cb200_mesh_set *m = io->meshes;
+    if (m->nodes == nullptr || m->triangles == nullptr || m->node_offset == nullptr || m->triangle_offset == nullptr ||
+        m->dims == nullptr || m->enable == nullptr || m->count == nullptr || (sp != nullptr && !expand) || io->dynamics != nullptr)
+      return ret(cudaErrorInvalidValue);
+    a.meshes = MeshSet{reinterpret_cast<const float4 *>(m->nodes), reinterpret_cast<const float4 *>(m->triangles), m->node_offset,
+                       m->triangle_offset, m->dims, m->inv_pose, m->enable, m->count, m->max_n, m->num_envs};
+  }
   if (expand) {
     // expanded schedule: knots -> state with the stand-alone spline kernel, then the plain rollout kernels read it
     const int rc = cb200_bspline_forward(sp->out_position, sp->out_velocity, sp->out_acceleration, sp->out_jerk, sp->out_dt,
@@ -3214,6 +3259,9 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
   // kernels are specialised on the obstacle types present (bit 0 cuboids, bit 1 voxel grids) so that e.g. the
   // IK kernel carries no ESDF code: the fused kernel's instruction footprint is what limits it.
   const int scene = (cfg->scene_weight > 0.0f ? ((a.cuboids.inv_pose ? 1 : 0) | (a.voxels.inv_pose ? 2 : 0)) : 0);
+  // Mesh scenes take one build per kernel family, SCENE = 7, which checks at run time whether cuboids and ESDF grids are
+  // present (5 kernels instead of 20 for SCENE in 4..7).  Cached launch plans of mesh scenes use slot 4.
+  const int sidx = mesh ? 4 : scene;
   using KernelT = void (*)(const FusedArgs);
   static KernelT const table[5][4] = {
       {rollout_fused_kernel<0, false>, rollout_fused_kernel<1, false>, rollout_fused_kernel<2, false>, rollout_fused_kernel<3, false>},
@@ -3240,7 +3288,7 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
     const char *e = getenv("CB200_LANE");
     return e ? atoi(e) : 0;  // off by default: measured slower than warp-per-row
   }();
-  if (!traj && lane_env != 0 && h.nl <= 24 && h.S <= 128 && a.spl.knots == nullptr && a.sphere_cfgs == nullptr) {
+  if (!traj && lane_env != 0 && !mesh && h.nl <= 24 && h.S <= 128 && a.spl.knots == nullptr && a.sphere_cfgs == nullptr) {
     static KernelT const lane_table[4] = {rollout_lane_kernel<0>, rollout_lane_kernel<1>, rollout_lane_kernel<2>,
                                           rollout_lane_kernel<3>};
     const LaneLayout ll = lane_layout(h.smem_bytes, kLaneThreads, h.nl, h.D, h.n_cl);
@@ -3271,7 +3319,7 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
     const char *e = getenv("CB200_TILE");
     return e ? atoi(e) : 0;
   }();
-  if (!traj && tile_env != 0 && a.spl.knots == nullptr && a.sphere_cfgs == nullptr) {
+  if (!traj && tile_env != 0 && !mesh && a.spl.knots == nullptr && a.sphere_cfgs == nullptr) {
     const TileLayout tl = tile_layout(h.smem_bytes, kWarpsPerCta, h.nl, h.D, h.S, h.L, h.n_cl);
     KernelT tk = table[2][scene];
     static thread_local size_t tile_cfg[4] = {0, 0, 0, 0};
@@ -3316,16 +3364,17 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
         {rollout_fused_big_kernel<0>, rollout_fused_big_kernel<1>, rollout_fused_big_kernel<2>, rollout_fused_big_kernel<3>},
         {rollout_fused_big_kernel<0, true>, rollout_fused_big_kernel<1, true>, rollout_fused_big_kernel<2, true>,
          rollout_fused_big_kernel<3, true>}};
+    static KernelT const big_mesh[2] = {rollout_fused_big_kernel<7>, rollout_fused_big_kernel<7, true>};
     const int small_arm = (h.nl <= 24 && h.S <= 128) ? 1 : 0;
     // (an 18-warp build -- 576 threads, 96 registers, small spills -- measured 0.237 ms on G1-29 against 0.219 ms for 16 warps)
     const int maxw = kBigWarps;
-    KernelT bk = big_table[small_arm][scene];
+    KernelT bk = mesh ? big_mesh[small_arm] : big_table[small_arm][scene];
     struct BigPlan {
       long long key = -1;
       int nw = 0, per_sm = 0;
     };
-    static thread_local BigPlan bplans[2][4];
-    BigPlan &bp = bplans[small_arm][scene];
+    static thread_local BigPlan bplans[2][5];
+    BigPlan &bp = bplans[small_arm][sidx];
     const int big_floats = big_smem_floats(h.nl, h.D, h.S, h.L, h.n_cl);
     const long long bkey = ((long long)h.smem_bytes << 32) ^ ((long long)big_floats << 8) ^ ((long long)(d.ordinal + 1) << 56);
     if (bkey != bp.key) {
@@ -3358,8 +3407,9 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
       }
     }
     // Small batches: a team of warps per row (rollout_fused_team_kernel) when the rows would leave at least half of the
-    // resident warp slots idle.  CB200_TEAM = 0 / 2 / 4 forces the team size.
-    {
+    // resident warp slots idle.  CB200_TEAM = 0 / 2 / 4 forces the team size.  The team kernel has no mesh build: mesh scenes
+    // stay on the big kernel.
+    if (!mesh) {
       const char *ts = getenv("CB200_TEAM");
       const int team_env = ts ? atoi(ts) : -1;
       const long long slots = (long long)d.sm_count * maxw;
@@ -3441,14 +3491,15 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
     }
   }
   int variant = (traj ? 1 : 0) + (a.spl.knots != nullptr ? 3 : 0);
-  KernelT kern = table[variant][scene];
+  static KernelT const mesh_table[2] = {rollout_fused_kernel<7, false>, rollout_traj_kernel<7, false>};  // (variant 0 / 1)
+  KernelT kern = mesh ? mesh_table[variant] : table[variant][scene];
   if (traj && h.nl <= 24 && h.S <= 128) {
     static KernelT const traj_small[2][4] = {
         {rollout_traj_kernel<0, false, true>, rollout_traj_kernel<1, false, true>, rollout_traj_kernel<2, false, true>,
          rollout_traj_kernel<3, false, true>},
         {rollout_traj_kernel<0, true, true>, rollout_traj_kernel<1, true, true>, rollout_traj_kernel<2, true, true>,
          rollout_traj_kernel<3, true, true>}};
-    kern = traj_small[a.spl.knots != nullptr ? 1 : 0][scene];
+    kern = mesh ? rollout_traj_kernel<7, false, true> : traj_small[a.spl.knots != nullptr ? 1 : 0][scene];
   }
   if (io->dynamics != nullptr) {
     // inverse dynamics inside the trajectory kernel: rows must come from caller-provided states (or the expanded spline
@@ -3516,8 +3567,10 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
   // H100 SXM at 400 W: 0.0183 vs 0.0255 ms at 1.0 rows per slot, 0.0274 vs 0.0270 ms at 1.5, 0.0324 vs 0.0271 ms at 2.0).  Not
   // against an ESDF: that build spills (140 B) and measured 2 % slower (franka_16384_esdf).  CB200_ARM_PAIRS = 0 / 1 forces one /
   // two rows per warp.
+  // Mesh scenes of arms stay on the 128-register build, one row per warp: an 80-register mesh build spilled 172 B (DESIGN.md
+  // section 4), so none is built.
   int rows_per_warp = 1;
-  if (variant == 0 && arm_regcap != 0 && (scene <= 1 || arm_esdf != 0) && h.nl <= 24 && h.S <= 128) {
+  if (variant == 0 && !mesh && arm_regcap != 0 && (scene <= 1 || arm_esdf != 0) && h.nl <= 24 && h.S <= 128) {
     const char *ps = getenv("CB200_ARM_PAIRS");  // read per call: tests switch it inside one process
     const int pairs_env = ps ? atoi(ps) : -1;
     const bool pairs = h.nl <= 16 && (scene & 2) == 0 &&
@@ -3528,15 +3581,15 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
     variant = pairs ? 6 : 5;
   }
   const int warp_floats = rows_per_warp * a.eval_floats;
-  const int minb = scene;  // part of the plan-cache key
+  const int minb = sidx;  // part of the plan-cache key
   // warps per CTA: the count that keeps the most warps resident per SM (shared memory is the limiter for
   // big robots); ties go to the larger CTA so the blob is staged fewer times.  Cached per (kernel, geometry).
   struct Plan {
     long long key = -1;
     int nw = 0, per_sm = 0;
   };
-  static thread_local Plan plans[7][4];
-  Plan &pl = plans[variant][scene];
+  static thread_local Plan plans[7][5];
+  Plan &pl = plans[variant][sidx];
   const size_t halo_bytes = traj ? (size_t)2 * h.S * sizeof(float4) : 0;
   const long long key = ((long long)h.smem_bytes << 32) ^ ((long long)warp_floats << 8) ^ (long long)minb ^
                         (traj ? ((long long)io->horizon << 40) : 0) ^ ((long long)(d.ordinal + 1) << 56);

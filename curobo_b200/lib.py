@@ -72,7 +72,8 @@ class RolloutIO(C.Structure):
                 ("batch_size", C.c_int32), ("horizon", C.c_int32), ("spline", C.POINTER(SplineInput)),
                 ("dynamics", C.POINTER(DynamicsParams)),
                 ("cspace_target", c_p), ("idxs_cspace_target", c_p), ("cspace_target_dof_weight", c_p),
-                ("sphere_configs", c_p), ("num_sphere_configs", C.c_int32), ("work_counter", c_p)]
+                ("sphere_configs", c_p), ("num_sphere_configs", C.c_int32), ("work_counter", c_p),
+                ("meshes", C.POINTER(MeshSet))]
 
 
 _I = C.c_int

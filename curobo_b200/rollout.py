@@ -20,6 +20,7 @@ from . import lib as _lib
 from .backends.tensor_checks import check_tensors, stream_ptr
 from .backends import tensor_checks as _tc
 from .robot_model import RobotModel
+from .mesh import c_mesh_set
 from .scene import CuboidData, VoxelData, c_cuboid_set, c_voxel_set
 
 
@@ -128,9 +129,14 @@ def pack_robot_blob(rm: RobotModel) -> np.ndarray:
 
 
 class RolloutEngine:
+    """`mesh` (curobo_b200.mesh.MeshData): triangle-mesh obstacles, evaluated inside the fused kernels next to the cuboids and
+    the ESDF grids.  In-place updates of its `inv_pose` / `enable` tensors take effect on the next call; a replaced MeshData
+    needs refresh_world().  Mesh scenes support every schedule except `evaluate_knots(in_kernel_spline=True)` and
+    `attach_dynamics(fused=True)`, which raise ValueError."""
+
     def __init__(self, robot: RobotModel, cfg: RolloutConfig, device="cuda:0",
                  cuboid: Optional[CuboidData] = None, voxel: Optional[VoxelData] = None,
-                 store_fk_outputs: bool = False, use_voxel_mip: bool = False):
+                 store_fk_outputs: bool = False, use_voxel_mip: bool = False, mesh=None):
         self.robot, self.cfg, self.device = robot, cfg, torch.device(device)
         _tc.require_cuda(self.device, "RolloutEngine is CUDA-only (sm_90a); there is no CPU path")
         self._lib = _lib.load()
@@ -141,7 +147,7 @@ class RolloutEngine:
         if robot.link_spheres.ndim == 3 and robot.link_spheres.shape[0] > 1:
             self._sphere_cfgs = torch.from_numpy(np.ascontiguousarray(robot.link_spheres, np.float32)).to(self.device)
         self._cs_target = None
-        self.cuboid, self.voxel = cuboid, voxel
+        self.cuboid, self.voxel, self.mesh = cuboid, voxel, mesh
         self.use_voxel_mip = use_voxel_mip
         self.refresh_world()
         self.store_fk_outputs = store_fk_outputs
@@ -185,8 +191,8 @@ class RolloutEngine:
                                               retime_regularization_weights=self.cfg.retime_reg)
 
     def refresh_world(self) -> None:
-        """Re-read the obstacle holders; call after the ESDF values (or obstacle tensors) were replaced or updated in
-        place.  With `use_voxel_mip=True` (opt-in) it rebuilds the ESDF lower-bound pyramid level (one tiny launch) that
+        """Re-read the obstacle holders (cuboids, ESDF grids, meshes); call after the ESDF values (or obstacle tensors) were
+        replaced or updated in place.  With `use_voxel_mip=True` (opt-in) it rebuilds the ESDF lower-bound pyramid level (one tiny launch) that
         lets discrete collision skip the corner fetches of samples that are provably inactive.  Exact while the level
         matches the grid: torch-side updates of `features` are detected (version stamp; the level is rebuilt on the next
         call), updates through raw pointers by foreign kernels are not -- call this after each of those."""
@@ -195,6 +201,7 @@ class RolloutEngine:
             build_voxel_mip(self.voxel)
         self._cs = c_cuboid_set(self.cuboid, self.device)
         self._vs = c_voxel_set(self.voxel, self.device)
+        self._ms = c_mesh_set(self.mesh, self.device)
         if self.voxel is not None and not self.use_voxel_mip and self._vs is not None:
             self._vs.mip, self._vs.mip_stride = None, 0
 
@@ -374,6 +381,8 @@ class RolloutEngine:
             io.cuboids = C.pointer(self._cs)
         if self._vs is not None:
             io.voxels = C.pointer(self._vs)
+        if self._ms is not None:
+            io.meshes = C.pointer(self._ms)
         if self.voxel is not None and self.use_voxel_mip:
             from .scene import voxel_mip_is_fresh
             if not voxel_mip_is_fresh(self.voxel):      # the ESDF tensor was updated or replaced since the level was built
@@ -417,6 +426,14 @@ class RolloutEngine:
         io.work_counter = self._work_counter.data_ptr()
         if self._dyn_params is not None and io.vel and io.acc and not bool(io.spline):
             io.dynamics = C.pointer(self._dyn_params)
+        if self._ms is not None and self.cfg.scene_weight > 0.0:
+            if io.dynamics:
+                raise ValueError("mesh obstacles are not supported by the dynamics-aware cost inside the kernel "
+                                 "(attach_dynamics(fused=True)); use attach_dynamics(fused=False), which adds the same terms "
+                                 "with separate launches")
+            if io.spline and not io.spline.contents.out_dt:
+                raise ValueError("mesh obstacles are not supported by the in-kernel spline schedule; use "
+                                 "evaluate_knots(in_kernel_spline=False), the expanded schedule")
         err = self._lib.cb200_rollout_cost_grad(C.byref(self._ccfg), C.byref(io), stream_ptr(dev))
         _lib.check(err, "rollout_cost_grad")
         return o

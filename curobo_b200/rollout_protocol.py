@@ -153,11 +153,12 @@ class B200RobotRollout:
 
     def __init__(self, robot: RobotModel, cfg: RolloutConfig, device="cuda:0", cuboid=None, voxel=None, horizon: int = 1,
                  dt: float = 0.05, action_space: str = "position", n_knots: int = 0, bspline_degree: int = 4,
-                 interpolation_steps: int = 4, sum_horizon: bool = True, use_voxel_mip: bool = False):
+                 interpolation_steps: int = 4, sum_horizon: bool = True, use_voxel_mip: bool = False, mesh=None):
         if action_space not in ("position", "bspline"):
             raise ValueError("action_space must be 'position' or 'bspline'")
         self.robot, self.cfg, self.device = robot, cfg, torch.device(device)
-        self.engine = RolloutEngine(robot, cfg, device, cuboid, voxel, store_fk_outputs=True, use_voxel_mip=use_voxel_mip)
+        self.engine = RolloutEngine(robot, cfg, device, cuboid, voxel, store_fk_outputs=True, use_voxel_mip=use_voxel_mip,
+                                    mesh=mesh)
         self.is_bspline = action_space == "bspline"
         self._degree, self._steps = bspline_degree, interpolation_steps
         if self.is_bspline:

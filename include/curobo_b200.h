@@ -351,6 +351,11 @@ typedef struct {
    * (the kernel re-arms it), owned by ONE stream at a time -- concurrent launches need one counter each.  Null: rows are
    * strided statically over the resident warps. */
   int32_t *work_counter;
+  /* Mesh obstacles, next to `cuboids` / `voxels` (host pointer to a struct of device pointers); NULL = none.  Read when
+   * cfg->scene_weight > 0 and meshes->inv_pose is set; discrete and swept collision against them run inside the fused kernels
+   * with the arithmetic of cb200_sphere_mesh_collision.  The in-kernel B-spline schedule and `dynamics` have no mesh support:
+   * with meshes present they return cudaErrorInvalidValue (the expanded spline schedule supports meshes). */
+  const cb200_mesh_set *meshes;
 } cb200_rollout_io;
 
 int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io *io,
