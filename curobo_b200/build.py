@@ -62,13 +62,11 @@ def _digest(paths) -> str:
     return h.hexdigest()
 
 
-def build_product(force: bool = False, verbose: bool = False, minb: int = 0) -> str:
-    """minb > 0 builds a tuning variant libcurobo_b200_mb<minb>.so (register cap = 65536 / (256 * minb)).
-    Up to date <=> the stamp next to the library holds the content hash of the sources (so an edited csrc/ never runs
+def build_product(force: bool = False, verbose: bool = False) -> str:
+    """Up to date <=> the stamp next to the library holds the content hash of the sources (so an edited csrc/ never runs
     a stale binary, and a fresh copy of the tree with new mtimes does not rebuild)."""
     srcs = [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC))] + [os.path.join(ROOT, "include", "curobo_b200.h")]
-    out = PRODUCT_SO if minb <= 0 else PRODUCT_SO.replace(".so", f"_mb{minb}.so")
-    stamp = out + ".stamp"
+    out, stamp = PRODUCT_SO, PRODUCT_SO + ".stamp"
     digest = _digest(srcs)
 
     def fresh() -> bool:
@@ -85,19 +83,18 @@ def build_product(force: bool = False, verbose: bool = False, minb: int = 0) -> 
     try:
         if not force and fresh():
             return out
-        return _build_product_locked(out, stamp, digest, verbose, minb)
+        return _build_product_locked(out, stamp, digest, verbose)
     finally:
         fcntl.flock(lock, fcntl.LOCK_UN)
         lock.close()
 
 
-def _build_product_locked(out: str, stamp: str, digest: str, verbose: bool, minb: int) -> str:
+def _build_product_locked(out: str, stamp: str, digest: str, verbose: bool) -> str:
     cmd = [_nvcc(), "-std=c++17", "-O3", "-lineinfo", *ARCH, *NUMERIC, "-Xcompiler", "-fPIC", "-shared",
-           "-Xptxas", "-v" if verbose else "-O3", *([f"-DCB200_MINB={minb}"] if minb > 0 else []),
-           "-o", out, "-lcudart"]
+           "-Xptxas", "-v" if verbose else "-O3", "-o", out, "-lcudart"]
     # three translation units (rollout, trajectory and optimizer kernels), compiled concurrently then linked
     units = ["cb200_kernels.cu", "cb200_trajectory.cu", "cb200_optim.cu", "cb200_dynamics.cu", "cb200_edt.cu"]
-    objs = [os.path.join(LIBDIR, (u[:-3] + (f"_mb{minb}" if minb > 0 else "") + ".o")) for u in units]
+    objs = [os.path.join(LIBDIR, u[:-3] + ".o") for u in units]
     flags = [c for c in cmd[1:] if c not in ("-shared", "-o", out, "-lcudart")]
     procs = [subprocess.Popen([cmd[0], *flags, "-c", os.path.join(CSRC, u), "-o", o], stdout=subprocess.PIPE,
                               stderr=subprocess.STDOUT, text=True) for u, o in zip(units, objs)]

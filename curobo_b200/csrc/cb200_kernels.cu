@@ -33,9 +33,7 @@ using namespace cb200;
 namespace {
 
 constexpr int kWarpsPerCta = 8;
-#ifndef CB200_MINB
-#define CB200_MINB 2  // CTAs/SM the register allocator must leave room for at 256 threads (tuning knob)
-#endif
+constexpr int kMinCtas = 2;  // CTAs/SM the register allocator must leave room for at 256 threads (the arm builds use 3)
 
 struct FusedArgs {
   cb200_rollout_cfg cfg;
@@ -53,7 +51,6 @@ struct FusedArgs {
   int32_t *pose_goalset_idx;
   int32_t B, H;
   int32_t blob_smem_bytes, eval_floats;
-  int32_t phase_sync;  // 0: warps free-run; 1: one CTA barrier per row (after phase A); 2: barrier after every phase
   // B-spline front end (8f-1): when spl.knots != nullptr the rows are the spline states of the knots and
   // q / vel / acc / jerk / dt above are not read
   struct Spline {
@@ -453,44 +450,12 @@ __device__ __forceinline__ void row_phase_b2(const FusedArgs &a, const RobotView
 
 // ------------------------------------------------------------------------------------------------
 // THE fused kernel, discrete scene collision: rows are independent, one persistent warp per row, phases
-// inlined (measured best).
+// inlined (measured best: out-of-line phases needed fewer registers and ran slower).
 // ------------------------------------------------------------------------------------------------
-#ifdef CB200_OOL_PHASES
-// Tuning variant (-DCB200_OOL_PHASES): out-of-line phase wrappers.  Each phase rebuilds its views from the blob
-// header in shared memory, so only a handful of values stay live across phases: 76 instead of ~113 registers,
-// but 84 us vs 82.7 us on the Franka IK workload, hence not the default.
-struct PhaseAOut {
-  float cs_cost, pose_c;
-};
-template <int W>
-static __device__ __noinline__ PhaseAOut phase_a_ool(const FusedArgs *a, const unsigned char *smem, float *base, int lane,
-                                                     int e, int b, int h) {
-  const RobotView rv = make_robot_view(smem, a->blob);
-  const EvalSmem es = carve_eval_smem(base, rv.nl, rv.D, rv.S, rv.L, rv.n_cl);
-  PhaseAOut o;
-  row_phase_a<false, W>(*a, rv, es, lane, e, b, h, o.cs_cost, o.pose_c);
-  return o;
-}
-template <int SCENE, int W>
-static __device__ __noinline__ RowB1 phase_b1_ool(const FusedArgs *a, const unsigned char *smem, float *base, int lane, int e,
-                                                  int b) {
-  const RobotView rv = make_robot_view(smem, a->blob);
-  const EvalSmem es = carve_eval_smem(base, rv.nl, rv.D, rv.S, rv.L, rv.n_cl);
-  return row_phase_b1<false, SCENE, W == 32, W>(*a, rv, es, lane, e, b, nullptr, nullptr);
-}
-template <int W>
-static __device__ __noinline__ void phase_b2_ool(const FusedArgs *a, const unsigned char *smem, float *base, int lane, int e,
-                                                 RowB1 r, float cs_cost, float pose_c) {
-  const RobotView rv = make_robot_view(smem, a->blob);
-  const EvalSmem es = carve_eval_smem(base, rv.nl, rv.D, rv.S, rv.L, rv.n_cl);
-  row_phase_b2<W == 16, W>(*a, rv, es, smem, lane, e, r, cs_cost, pose_c);
-}
-#endif  // CB200_OOL_PHASES
-
 // ROWS = 2 (arm build only, robots of <= 16 links): two rows per warp, half h = lane >> 4 owns row 2 u + h of the warp's work
 // unit u, with the row helpers at width 16.  The halves run the same code on different rows and may diverge inside a row; they
 // meet again at the end of it, where the next unit is fetched.  A row's result does not depend on its partner.
-template <int SCENE, bool SPLINE, int MINB = CB200_MINB, int ROWS = 1>
+template <int SCENE, bool SPLINE, int MINB = kMinCtas, int ROWS = 1>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB) rollout_fused_kernel(const __grid_constant__ FusedArgs a) {
   static_assert(ROWS == 1 || (ROWS == 2 && MINB == 3 && !SPLINE), "paired rows: arm build only");
   constexpr int W = 32 / ROWS;
@@ -515,18 +480,12 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB) rollout_fused_kernel(
         b = e / a.H;
         h = e - b * a.H;
       }
-#ifndef CB200_OOL_PHASES
       const RobotView rv = make_robot_view(smem, a.blob);
       const EvalSmem es = carve_eval_smem(base, rv.nl, rv.D, rv.S, rv.L, rv.n_cl);
       float cs_cost = 0.0f, pose_c = 0.0f;
       row_phase_a<SPLINE, W>(a, rv, es, lane, e, b, h, cs_cost, pose_c);
       const RowB1 r = row_phase_b1<false, SCENE, MINB != 3, W>(a, rv, es, lane, e, b, nullptr, nullptr);
       row_phase_b2<MINB == 3, W>(a, rv, es, smem, lane, e, r, cs_cost, pose_c);
-#else
-      const PhaseAOut pa = phase_a_ool<W>(&a, smem, base, lane, e, b, h);
-      const RowB1 r = phase_b1_ool<SCENE, W>(&a, smem, base, lane, e, b);
-      phase_b2_ool<W>(&a, smem, base, lane, e, r, pa.cs_cost, pa.pose_c);
-#endif
     }
     if (a.work_counter != nullptr) {
       int nxt = 0;
@@ -1082,7 +1041,7 @@ __global__ void __launch_bounds__(kBigWarps * 32, 1) rollout_fused_team_kernel(c
 // ------------------------------------------------------------------------------------------------
 // SMALL: arms (<= 24 links, <= 128 spheres): whole-block self-collision scan and the one-slot sparse J^T (see the IK arm build).
 template <int SCENE, bool SPLINE, bool SMALL = false>
-__global__ void __launch_bounds__(kWarpsPerCta * 32, CB200_MINB) rollout_traj_kernel(const __grid_constant__ FusedArgs a) {
+__global__ void __launch_bounds__(kWarpsPerCta * 32, kMinCtas) rollout_traj_kernel(const __grid_constant__ FusedArgs a) {
   CB200_EXTERN_SHARED __align__(128) unsigned char smem[];
   __shared__ unsigned long long mbar;
   stage_blob_to_smem(smem, a.blob, (uint32_t)a.blob_smem_bytes, &mbar);
@@ -1171,7 +1130,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, CB200_MINB) rollout_traj_ke
 // dynamics of a chunk is ~32 k warp-instructions, which a single warp issues more slowly than eight warps roll the chunk out.
 // ------------------------------------------------------------------------------------------------
 template <int SCENE>
-__global__ void __launch_bounds__(kWarpsPerCta * 32, CB200_MINB) rollout_traj_dyn_kernel(const __grid_constant__ FusedArgs a,
+__global__ void __launch_bounds__(kWarpsPerCta * 32, kMinCtas) rollout_traj_dyn_kernel(const __grid_constant__ FusedArgs a,
                                                                                          const int R) {
   CB200_EXTERN_SHARED __align__(128) unsigned char smem[];
   __shared__ unsigned long long mbar;
@@ -1293,618 +1252,6 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, CB200_MINB) rollout_traj_dy
       if (active) row_phase_b2(a, rv, es, smem, lane, e, r, cs_cost, pose_c);
     }
     __syncthreads();  // the next chunk's dynamics phase rewrites the tile the last rows just read
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// THE fused kernel for small robots (arms): "tile" schedule.
-//
-// The serial, scalar parts of a row -- the FK chain, the tool-pose cost, the c-space cost and the J^T
-// up-sweep -- use 1..24 of 32 lanes when a warp owns a row and they are ~60 % of the
-// instructions.  Here a CTA owns a tile of T = 8 warps x 8 rows and alternates between two mappings:
-//   phase 1  thread per row  (T threads): q, c-space, FK chain in registers -> cumul[T] in shared memory,
-//                                         tool poses + tool-pose cost
-//   phase 2  warp per row    (8 warps x 8 rows each): spheres, self collision (broad phase + tiles),
-//                                         scene collision, sparse reduction of the sphere gradients to
-//                                         per-link force / torque accumulators
-//   phase 3  thread per row  (T threads): tool-frame gradients, subtree up-sweep of (F, T) in reverse link
-//                                         order, joint gradients, grad_q and row cost
-// Rows in shared memory are laid out row-major with a stride = 4 (mod 32) floats so that 128-bit accesses of
-// consecutive threads (phase 1/3) are bank-conflict free, and a warp reading one row (phase 2) uses float4.
-// ------------------------------------------------------------------------------------------------
-constexpr int kTileEpw = 8;  // rows per warp in phase 2
-
-__host__ __device__ inline int tile_stride(int floats) {  // smallest s >= floats with s % 32 == 4
-  int s = ((floats + 27) / 32) * 32 + 4;
-  return s;
-}
-
-struct TileLayout {
-  int T, cstride, fstride;
-  size_t off_scratch, scratch_floats, off_cum, off_ft, off_q, off_gq, off_pose, off_selfc, off_scenec, total_bytes;
-};
-__host__ __device__ inline TileLayout tile_layout(int blob_smem_bytes, int nwarps, int nl, int D, int S, int L, int n_cl) {
-  TileLayout t;
-  t.T = nwarps * kTileEpw;
-  t.cstride = tile_stride(nl * 12);
-  t.fstride = tile_stride(nl * 8);
-  size_t off = (size_t)blob_smem_bytes;
-  t.off_scratch = off;
-  t.scratch_floats = (size_t)(2 * S + n_cl) * 4 + (size_t)((n_cl + 3) & ~3);
-  off += (size_t)nwarps * t.scratch_floats * 4;
-  t.off_cum = off;
-  off += (size_t)t.T * t.cstride * 4;
-  t.off_ft = off;
-  off += (size_t)t.T * t.fstride * 4;
-  t.off_q = off;
-  off += (size_t)D * t.T * 4;
-  t.off_gq = off;
-  off += (size_t)D * t.T * 4;
-  t.off_pose = off;
-  off += (size_t)L * 8 * t.T * 4;
-  t.off_selfc = off;
-  off += (size_t)t.T * 4;
-  t.off_scenec = off;
-  off += (size_t)t.T * 4;
-  t.total_bytes = (off + 15) & ~(size_t)15;
-  return t;
-}
-
-template <int SCENE>
-__global__ void __launch_bounds__(kWarpsPerCta * 32, 2) rollout_tile_kernel(const __grid_constant__ FusedArgs a) {
-  CB200_EXTERN_SHARED __align__(128) unsigned char smem[];
-  __shared__ unsigned long long mbar;
-  stage_blob_to_smem(smem, a.blob, (uint32_t)a.blob_smem_bytes, &mbar);
-  const RobotView rv = make_robot_view(smem, a.blob);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  const TileLayout tl = tile_layout(a.blob_smem_bytes, nwarps, rv.nl, rv.D, rv.S, rv.L, rv.n_cl);
-  const int T = tl.T, D = rv.D, S = rv.S, L = rv.L, nl = rv.nl;
-  float *scratch = reinterpret_cast<float *>(smem + tl.off_scratch) + (size_t)warp * tl.scratch_floats;
-  float *cum = reinterpret_cast<float *>(smem + tl.off_cum);
-  float *ftb = reinterpret_cast<float *>(smem + tl.off_ft);
-  float *qs = reinterpret_cast<float *>(smem + tl.off_q);
-  float *gqs = reinterpret_cast<float *>(smem + tl.off_gq);
-  float *pose_g = reinterpret_cast<float *>(smem + tl.off_pose);
-  float *selfc = reinterpret_cast<float *>(smem + tl.off_selfc);
-  float *scenec = reinterpret_cast<float *>(smem + tl.off_scenec);
-  EvalSmem es;  // phase-2 view: cumul points at the current row, the rest is this warp's scratch
-  es.sph = reinterpret_cast<float4 *>(scratch);
-  es.gsph = es.sph + S;
-  es.bc = es.gsph + S;
-  es.cmask = reinterpret_cast<uint32_t *>(es.bc + rv.n_cl);
-  es.cumul = es.ft = es.contrib = es.qv = es.gqv = es.pose_g = nullptr;
-  const cb200_rollout_cfg &cfg = a.cfg;
-  const int N = a.B * a.H;
-  const int n_tiles = (N + T - 1) / T;
-  const int t = threadIdx.x;
-  const bool do_pose = (a.goal_position != nullptr);
-
-  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const int tile_base = tile * T;
-    // ---------------- phase 1: thread per row
-    float cs_cost = 0.0f, pose_c = 0.0f;
-    const int e1 = tile_base + t;
-    const bool act1 = (t < T) && (e1 < N);
-    if (act1) {
-      const int b = e1 / a.H, h = e1 - b * a.H;
-#pragma unroll 1
-      for (int d = 0; d < D; ++d) {
-        const bspline::State4 st = load_row_state<false>(a, e1, b, h, d, D);
-        qs[d * T + t] = st.p;
-        float gp;
-        const float c = cspace_dof(a, rv, e1, b, h, d, st, gp);
-        gqs[d * T + t] = gp;
-        cs_cost += c;
-        if (a.cspace_cost) a.cspace_cost[(size_t)e1 * D + d] = c;
-      }
-      float *C = cum + (size_t)t * tl.cstride;
-#pragma unroll 1
-      for (int l = 0; l < nl; ++l) {
-        const int jt = rv.joint_type[l];
-        float th = 0.0f;
-        if (jt >= 0) th = rv.joff[2 * l] * qs[rv.joint_map[l] * T + t] + rv.joff[2 * l + 1];
-        float m[12];
-        local_link_transform(rv.fixed + 12 * l, jt, th, m);
-        float4 o0, o1, o2;
-        if (l == 0) {
-          o0 = make_float4(m[0], m[1], m[2], m[3]);
-          o1 = make_float4(m[4], m[5], m[6], m[7]);
-          o2 = make_float4(m[8], m[9], m[10], m[11]);
-        } else {
-          const float4 *P = reinterpret_cast<const float4 *>(C + 12 * rv.link_map[l]);
-          const float4 p0 = P[0], p1 = P[1], p2 = P[2];
-          o0 = make_float4(p0.x * m[0] + p0.y * m[4] + p0.z * m[8], p0.x * m[1] + p0.y * m[5] + p0.z * m[9],
-                           p0.x * m[2] + p0.y * m[6] + p0.z * m[10], p0.x * m[3] + p0.y * m[7] + p0.z * m[11] + p0.w);
-          o1 = make_float4(p1.x * m[0] + p1.y * m[4] + p1.z * m[8], p1.x * m[1] + p1.y * m[5] + p1.z * m[9],
-                           p1.x * m[2] + p1.y * m[6] + p1.z * m[10], p1.x * m[3] + p1.y * m[7] + p1.z * m[11] + p1.w);
-          o2 = make_float4(p2.x * m[0] + p2.y * m[4] + p2.z * m[8], p2.x * m[1] + p2.y * m[5] + p2.z * m[9],
-                           p2.x * m[2] + p2.y * m[6] + p2.z * m[10], p2.x * m[3] + p2.y * m[7] + p2.z * m[11] + p2.w);
-        }
-        float4 *O = reinterpret_cast<float4 *>(C + 12 * l);
-        O[0] = o0;
-        O[1] = o1;
-        O[2] = o2;
-      }
-#pragma unroll 1
-      for (int tf = 0; tf < L; ++tf) {
-        const float *Tm = C + 12 * rv.tool_map[tf];
-        const V3 p = mk3(Tm[3], Tm[7], Tm[11]);
-        const Q4 qt = quat_from_transform(Tm);
-        if (a.link_pos) {
-          float *o = a.link_pos + ((size_t)e1 * L + tf) * 3;
-          o[0] = p.x;
-          o[1] = p.y;
-          o[2] = p.z;
-        }
-        if (a.link_quat) *reinterpret_cast<float4 *>(a.link_quat + ((size_t)e1 * L + tf) * 4) = make_float4(qt.w, qt.x, qt.y, qt.z);
-        V3 gpos = mk3(0, 0, 0), om = mk3(0, 0, 0);
-        if (do_pose) {
-          const int gi = a.idxs_goal ? __ldg(a.idxs_goal + b) : 0;
-          const bool term = !(h < a.H - 1 && a.H > 1);
-          const float *axes = term ? a.pose_axes_t : a.pose_axes_nt;
-          const float *tol = term ? a.pose_tol_t : a.pose_tol_nt;
-          const size_t go = ((size_t)gi * L + tf) * cfg.num_goalset;
-          const PoseOut po = tool_pose_cost(p, qt, a.goal_position + go * 3, a.goal_quat + go * 4, cfg.num_goalset,
-                                            cfg.pose_weight[0], cfg.pose_weight[1], axes, tf,
-                                            tol != nullptr ? __ldg(tol + 2 * tf) : 0.0f,
-                                            tol != nullptr ? __ldg(tol + 2 * tf + 1) : 0.0f, cfg.pose_rotation_method);
-          om = quat_grad_to_omega(qt, po.gq_w, po.gq_x, po.gq_y, po.gq_z);
-          gpos = po.g_pos;
-          pose_c += po.pos_cost + po.rot_cost;
-          if (a.pose_cost) {
-            a.pose_cost[((size_t)e1 * L + tf) * 2] = po.pos_cost;
-            a.pose_cost[((size_t)e1 * L + tf) * 2 + 1] = po.rot_cost;
-          }
-          if (a.pose_goalset_idx) a.pose_goalset_idx[(size_t)e1 * L + tf] = po.goal_idx;
-        }
-        float *pg = pose_g + (size_t)tf * 8 * T + t;
-        pg[0 * T] = gpos.x;
-        pg[1 * T] = gpos.y;
-        pg[2 * T] = gpos.z;
-        pg[4 * T] = om.x;
-        pg[5 * T] = om.y;
-        pg[6 * T] = om.z;
-      }
-    }
-    __syncthreads();
-    // ---------------- phase 2: warp per row
-#pragma unroll 1
-    for (int i = 0; i < kTileEpw; ++i) {
-      const int ti = warp * kTileEpw + i;
-      const int e = tile_base + ti;
-      if (e >= N) break;  // warp-uniform
-      const int b = e / a.H;
-      es.cumul = cum + (size_t)ti * tl.cstride;
-      float *FT = ftb + (size_t)ti * tl.fstride;
-      warp_spheres(rv, es, lane, a.robot_spheres ? reinterpret_cast<float4 *>(a.robot_spheres) + (size_t)e * S : nullptr);
-      for (int k = lane; k < nl * 2; k += 32) reinterpret_cast<float4 *>(FT)[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-      __syncwarp();
-      const RowB1 r = row_phase_b1<false, SCENE>(a, rv, es, lane, e, b, nullptr, nullptr);
-      if (r.fmax > 0.0f && lane == 0) {
-        const float4 pi = es.sph[r.bi], pj = es.sph[r.bj];
-        const float w = cfg.self_weight;
-        float4 gi = es.gsph[r.bi], gj = es.gsph[r.bj];
-        const float gx = w * (pj.x - pi.x), gy = w * (pj.y - pi.y), gz = w * (pj.z - pi.z);
-        gi.x += gx;
-        gi.y += gy;
-        gi.z += gz;
-        gj.x -= gx;
-        gj.y -= gy;
-        gj.z -= gz;
-        es.gsph[r.bi] = gi;
-        es.gsph[r.bj] = gj;
-      }
-      __syncwarp();
-      // sparse reduction of the sphere gradients to per-link (F, T about the link origin)
-#pragma unroll 1
-      for (int base = 0; base < S; base += 32) {
-        const int s = base + lane;
-        bool nz = false;
-        if (s < S) {
-          const float4 g = es.gsph[s];
-          nz = (g.x != 0.0f) || (g.y != 0.0f) || (g.z != 0.0f);
-        }
-        unsigned m = __ballot_sync(kFull, nz);
-        while (m) {
-          const int ss = base + __ffs(m) - 1;
-          m &= m - 1;
-          const float4 g4 = es.gsph[ss], p4 = es.sph[ss];
-          const int k = rv.sph_link[ss];
-          const float *Tk = es.cumul + 12 * k;
-          const V3 g = mk3(g4.x, g4.y, g4.z);
-          const V3 tq = cross(mk3(p4.x - Tk[3], p4.y - Tk[7], p4.z - Tk[11]), g);
-          if (lane < 6) {
-            const float v = lane == 0 ? g.x : lane == 1 ? g.y : lane == 2 ? g.z : lane == 3 ? tq.x : lane == 4 ? tq.y : tq.z;
-            FT[8 * k + lane + (lane >= 3 ? 1 : 0)] += v;
-          }
-          __syncwarp();
-        }
-      }
-      const float sc = warp_sum(r.scene_c);
-      if (lane == 0) {
-        selfc[ti] = r.self_c;
-        scenec[ti] = sc;
-      }
-      __syncwarp();
-    }
-    __syncthreads();
-    // ---------------- phase 3: thread per row
-    if (act1) {
-      const float *C = cum + (size_t)t * tl.cstride;
-      float *FT = ftb + (size_t)t * tl.fstride;
-#pragma unroll 1
-      for (int tf = 0; tf < L; ++tf) {
-        const float *pg = pose_g + (size_t)tf * 8 * T + t;
-        float4 *Fk = reinterpret_cast<float4 *>(FT + 8 * rv.tool_map[tf]);
-        float4 f = Fk[0], tq = Fk[1];
-        f.x += pg[0 * T];
-        f.y += pg[1 * T];
-        f.z += pg[2 * T];
-        tq.x += pg[4 * T];
-        tq.y += pg[5 * T];
-        tq.z += pg[6 * T];
-        Fk[0] = f;
-        Fk[1] = tq;
-      }
-#pragma unroll 1
-      for (int l = nl - 1; l >= 1; --l) {
-        const int p = rv.link_map[l];
-        const float4 f = reinterpret_cast<const float4 *>(FT + 8 * l)[0], tq = reinterpret_cast<const float4 *>(FT + 8 * l)[1];
-        const float *Tl = C + 12 * l, *Tp = C + 12 * p;
-        const V3 dxo = mk3(Tl[3] - Tp[3], Tl[7] - Tp[7], Tl[11] - Tp[11]);
-        const V3 cr = cross(dxo, mk3(f.x, f.y, f.z));
-        float4 *Fp = reinterpret_cast<float4 *>(FT + 8 * p);
-        float4 fp = Fp[0], tp = Fp[1];
-        fp.x += f.x;
-        fp.y += f.y;
-        fp.z += f.z;
-        tp.x += tq.x + cr.x;
-        tp.y += tq.y + cr.y;
-        tp.z += tq.z + cr.z;
-        Fp[0] = fp;
-        Fp[1] = tp;
-      }
-#pragma unroll 1
-      for (int l = 0; l < nl; ++l) {
-        const int jt = rv.joint_type[l];
-        if (jt < 0) continue;
-        const float *Tl = C + 12 * l;
-        const int ax = (jt >= JT_XR) ? jt - JT_XR : jt;
-        const V3 av = mk3(Tl[ax], Tl[4 + ax], Tl[8 + ax]);
-        const float4 w = reinterpret_cast<const float4 *>(FT + 8 * l)[(jt >= JT_XR) ? 1 : 0];
-        gqs[rv.joint_map[l] * T + t] += rv.joff[2 * l] * (av.x * w.x + av.y * w.y + av.z * w.z);
-      }
-#pragma unroll 1
-      for (int d = 0; d < D; ++d) a.grad_q[(size_t)e1 * D + d] = gqs[d * T + t];
-      a.cost[e1] = cs_cost + pose_c + scenec[t] + selfc[t];
-    }
-    __syncthreads();
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// THE fused kernel for small robots, "lane" schedule: ONE THREAD PER ROW for the whole row.
-//
-// Profiles r01_a/b: with a warp per row, 60 % of the instructions run with 1..24 of 32 lanes (FK chain,
-// tool-pose cost, J^T walk) and the warp-level barriers/shuffles chain their latencies.  For an arm
-// (13 links, 65 spheres) a row is small enough for one thread: 32 rows per warp run in lock-step with every
-// lane busy, no barrier, no shuffle, and no intermediate ever leaves the thread except the link transforms
-// (shared memory, private column per thread).  Two exact broad phases keep the per-thread work small:
-//   self collision: link x link bounding spheres (same test as warp_self_collision_tiles);
-//   cuboids       : a box SDF is 1-Lipschitz, so if sdf(link bound centre) >= R_link + eta no sphere of the
-//                   link can have pen = r + eta - sdf > 0 against that cuboid.
-// Gradients go straight to joint space: every colliding sphere / tool frame walks its ancestor links.
-// ------------------------------------------------------------------------------------------------
-struct LaneLayout {
-  int cstride, bstride;  // floats per thread for cumul / link bounds, both = 4 (mod 32)
-  size_t off_cum, off_bc, off_q, off_gq, total_bytes;
-};
-__host__ __device__ inline LaneLayout lane_layout(int blob_smem_bytes, int T, int nl, int D, int n_cl) {
-  LaneLayout t;
-  t.cstride = tile_stride(nl * 12);
-  t.bstride = tile_stride((n_cl > 0 ? n_cl : 1) * 4);
-  size_t off = (size_t)blob_smem_bytes;
-  t.off_cum = off;
-  off += (size_t)T * t.cstride * 4;
-  t.off_bc = off;
-  off += (size_t)T * t.bstride * 4;
-  t.off_q = off;
-  off += (size_t)D * T * 4;
-  t.off_gq = off;
-  off += (size_t)D * T * 4;
-  t.total_bytes = (off + 15) & ~(size_t)15;
-  return t;
-}
-
-__device__ __forceinline__ V3 xf_point(const float *T, float x, float y, float z) {
-  const float4 r0 = *reinterpret_cast<const float4 *>(T), r1 = *reinterpret_cast<const float4 *>(T + 4),
-               r2 = *reinterpret_cast<const float4 *>(T + 8);
-  return mk3(r0.x * x + r0.y * y + r0.z * z + r0.w, r1.x * x + r1.y * y + r1.z * z + r1.w,
-             r2.x * x + r2.y * y + r2.z * z + r2.w);
-}
-
-constexpr int kLaneThreads = 64;
-
-template <int SCENE>
-__global__ void __launch_bounds__(kLaneThreads, 4) rollout_lane_kernel(const __grid_constant__ FusedArgs a) {
-  CB200_EXTERN_SHARED __align__(128) unsigned char smem[];
-  __shared__ unsigned long long mbar;
-  stage_blob_to_smem(smem, a.blob, (uint32_t)a.blob_smem_bytes, &mbar);
-  const RobotView rv = make_robot_view(smem, a.blob);
-  const int t = threadIdx.x, T = blockDim.x;
-  const LaneLayout ll = lane_layout(a.blob_smem_bytes, T, rv.nl, rv.D, rv.n_cl);
-  float *C = reinterpret_cast<float *>(smem + ll.off_cum) + (size_t)t * ll.cstride;
-  float4 *BC = reinterpret_cast<float4 *>(reinterpret_cast<float *>(smem + ll.off_bc) + (size_t)t * ll.bstride);
-  float *qs = reinterpret_cast<float *>(smem + ll.off_q) + t;    // [d * T]
-  float *gqs = reinterpret_cast<float *>(smem + ll.off_gq) + t;  // [d * T]
-  const cb200_rollout_cfg &cfg = a.cfg;
-  const int D = rv.D, S = rv.S, L = rv.L, nl = rv.nl;
-  const int N = a.B * a.H;
-  const bool do_pose = (a.goal_position != nullptr);
-  const bool do_scene = SCENE != 0 && cfg.scene_weight > 0.0f;
-
-  // ancestors of link k: add  s * a_j . ((p - o_j) x g + om)  (revolute) / s * a_j . g (prismatic) to joint(j)
-  auto chain_add = [&](int k, V3 p, V3 g, V3 om) {
-    unsigned long long m = rv.anc_mask[k];
-    while (m) {
-      const int j = __ffsll((long long)m) - 1;
-      m &= m - 1;
-      const int jt = rv.joint_type[j];
-      if (jt < 0) continue;
-      const float *Tj = C + 12 * j;
-      const int ax = (jt >= JT_XR) ? jt - JT_XR : jt;
-      const V3 av = mk3(Tj[ax], Tj[4 + ax], Tj[8 + ax]);
-      float v;
-      if (jt >= JT_XR) {
-        v = dot(av, cross(mk3(p.x - Tj[3], p.y - Tj[7], p.z - Tj[11]), g) + om);
-      } else {
-        v = dot(av, g);
-      }
-      gqs[rv.joint_map[j] * T] += rv.joff[2 * j] * v;
-    }
-  };
-
-#pragma unroll 1
-  for (int e = blockIdx.x * T + t; e < N; e += gridDim.x * T) {
-    const int b = e / a.H, h = e - b * a.H;
-    // ---- q, c-space
-    float cs_cost = 0.0f;
-#pragma unroll 4
-    for (int d = 0; d < D; ++d) {
-      const bspline::State4 st = load_row_state<false>(a, e, b, h, d, D);
-      qs[d * T] = st.p;
-      float gp;
-      const float c = cspace_dof(a, rv, e, b, h, d, st, gp);
-      gqs[d * T] = gp;
-      cs_cost += c;
-      if (a.cspace_cost) a.cspace_cost[(size_t)e * D + d] = c;
-    }
-    // ---- FK chain
-#pragma unroll 1
-    for (int l = 0; l < nl; ++l) {
-      const int jt = rv.joint_type[l];
-      float th = 0.0f;
-      if (jt >= 0) th = rv.joff[2 * l] * qs[rv.joint_map[l] * T] + rv.joff[2 * l + 1];
-      float m[12];
-      local_link_transform(rv.fixed + 12 * l, jt, th, m);
-      float4 o0, o1, o2;
-      if (l == 0) {
-        o0 = make_float4(m[0], m[1], m[2], m[3]);
-        o1 = make_float4(m[4], m[5], m[6], m[7]);
-        o2 = make_float4(m[8], m[9], m[10], m[11]);
-      } else {
-        const float4 *P = reinterpret_cast<const float4 *>(C + 12 * rv.link_map[l]);
-        const float4 p0 = P[0], p1 = P[1], p2 = P[2];
-        o0 = make_float4(p0.x * m[0] + p0.y * m[4] + p0.z * m[8], p0.x * m[1] + p0.y * m[5] + p0.z * m[9],
-                         p0.x * m[2] + p0.y * m[6] + p0.z * m[10], p0.x * m[3] + p0.y * m[7] + p0.z * m[11] + p0.w);
-        o1 = make_float4(p1.x * m[0] + p1.y * m[4] + p1.z * m[8], p1.x * m[1] + p1.y * m[5] + p1.z * m[9],
-                         p1.x * m[2] + p1.y * m[6] + p1.z * m[10], p1.x * m[3] + p1.y * m[7] + p1.z * m[11] + p1.w);
-        o2 = make_float4(p2.x * m[0] + p2.y * m[4] + p2.z * m[8], p2.x * m[1] + p2.y * m[5] + p2.z * m[9],
-                         p2.x * m[2] + p2.y * m[6] + p2.z * m[10], p2.x * m[3] + p2.y * m[7] + p2.z * m[11] + p2.w);
-      }
-      float4 *O = reinterpret_cast<float4 *>(C + 12 * l);
-      O[0] = o0;
-      O[1] = o1;
-      O[2] = o2;
-    }
-    // ---- tool poses + tool-pose cost (gradient walks the chain immediately)
-    float pose_c = 0.0f;
-#pragma unroll 1
-    for (int tf = 0; tf < L; ++tf) {
-      const int k = rv.tool_map[tf];
-      const float *Tm = C + 12 * k;
-      const V3 p = mk3(Tm[3], Tm[7], Tm[11]);
-      const Q4 qt = quat_from_transform(Tm);
-      if (a.link_pos) {
-        float *o = a.link_pos + ((size_t)e * L + tf) * 3;
-        o[0] = p.x;
-        o[1] = p.y;
-        o[2] = p.z;
-      }
-      if (a.link_quat) *reinterpret_cast<float4 *>(a.link_quat + ((size_t)e * L + tf) * 4) = make_float4(qt.w, qt.x, qt.y, qt.z);
-      if (do_pose) {
-        const int gi = a.idxs_goal ? __ldg(a.idxs_goal + b) : 0;
-        const bool term = !(h < a.H - 1 && a.H > 1);
-        const float *axes = term ? a.pose_axes_t : a.pose_axes_nt;
-        const float *tol = term ? a.pose_tol_t : a.pose_tol_nt;
-        const size_t go = ((size_t)gi * L + tf) * cfg.num_goalset;
-        const PoseOut po = tool_pose_cost(p, qt, a.goal_position + go * 3, a.goal_quat + go * 4, cfg.num_goalset,
-                                          cfg.pose_weight[0], cfg.pose_weight[1], axes, tf,
-                                          tol != nullptr ? __ldg(tol + 2 * tf) : 0.0f,
-                                          tol != nullptr ? __ldg(tol + 2 * tf + 1) : 0.0f, cfg.pose_rotation_method);
-        const V3 om = quat_grad_to_omega(qt, po.gq_w, po.gq_x, po.gq_y, po.gq_z);
-        pose_c += po.pos_cost + po.rot_cost;
-        if (a.pose_cost) {
-          a.pose_cost[((size_t)e * L + tf) * 2] = po.pos_cost;
-          a.pose_cost[((size_t)e * L + tf) * 2 + 1] = po.rot_cost;
-        }
-        if (a.pose_goalset_idx) a.pose_goalset_idx[(size_t)e * L + tf] = po.goal_idx;
-        const bool nzg = po.g_pos.x != 0.0f || po.g_pos.y != 0.0f || po.g_pos.z != 0.0f || om.x != 0.0f || om.y != 0.0f || om.z != 0.0f;
-        if (nzg) chain_add(k, p, po.g_pos, om);
-      }
-    }
-    // ---- self collision
-    float self_c = 0.0f;
-    if (cfg.self_weight > 0.0f && rv.P > 0) {
-      float best = 0.0f;
-      int bi = 0, bj = 0;
-      if (rv.n_lp > 0) {
-#pragma unroll 4
-        for (int ca = 0; ca < rv.n_cl; ++ca) {
-          const float4 c = rv.cl_bound[ca];
-          const V3 w = xf_point(C + 12 * rv.cl_link[ca], c.x, c.y, c.z);
-          BC[ca] = make_float4(w.x, w.y, w.z, c.w);
-        }
-#pragma unroll 4
-        for (int p = 0; p < rv.n_lp; ++p) {
-          const uint32_t pr = rv.lp[p];
-          const int la = pr & 0xffffu, lb = pr >> 16;
-          const float4 A = BC[la], Bq = BC[lb];
-          const float dx = A.x - Bq.x, dy = A.y - Bq.y, dz = A.z - Bq.z, rs = A.w + Bq.w;
-          if (!((A.w >= 0.0f) && (Bq.w >= 0.0f) && (dx * dx + dy * dy + dz * dz < rs * rs))) continue;
-          const float *Ta = C + 12 * rv.cl_link[la], *Tb = C + 12 * rv.cl_link[lb];
-#pragma unroll 2
-          for (int i = rv.cl_start[la]; i < rv.cl_start[la + 1]; ++i) {
-            const float4 si = rv.spheres[i];
-            const float ri = si.w + rv.padding[i];
-            if (!(ri >= 0.0f)) continue;
-            const V3 pi = xf_point(Ta, si.x, si.y, si.z);
-#pragma unroll 4
-            for (int j = rv.cl_start[lb]; j < rv.cl_start[lb + 1]; ++j) {
-              const float4 sj = rv.spheres[j];
-              const float rj = sj.w + rv.padding[j];
-              if (!(rj >= 0.0f)) continue;
-              const V3 pj = xf_point(Tb, sj.x, sj.y, sj.z);
-              const float rr = ri + rj, ex = pi.x - pj.x, ey = pi.y - pj.y, ez = pi.z - pj.z;
-              const float f = rr * rr - (ex * ex + ey * ey + ez * ez);
-              // arg-max with ties to the first pair in list order = smallest (i, j)
-              if (f > best || (f == best && f > 0.0f && (i < bi || (i == bi && j < bj)))) {
-                best = f;
-                bi = i;
-                bj = j;
-              }
-            }
-          }
-        }
-      } else {
-#pragma unroll 1
-        for (int p = 0; p < rv.P; ++p) {  // explicit pair list (not a union of link blocks)
-          const uint32_t pr = __ldg(rv.pairs + p);
-          const int i = pr & 0xffffu, j = pr >> 16;
-          const float4 si = rv.spheres[i], sj = rv.spheres[j];
-          const float ri = si.w + rv.padding[i], rj = sj.w + rv.padding[j];
-          if (!(ri >= 0.0f && rj >= 0.0f)) continue;
-          const V3 pi = xf_point(C + 12 * rv.sph_link[i], si.x, si.y, si.z);
-          const V3 pj = xf_point(C + 12 * rv.sph_link[j], sj.x, sj.y, sj.z);
-          const float rr = ri + rj, ex = pi.x - pj.x, ey = pi.y - pj.y, ez = pi.z - pj.z;
-          const float f = rr * rr - (ex * ex + ey * ey + ez * ez);
-          if (f > best) {
-            best = f;
-            bi = i;
-            bj = j;
-          }
-        }
-      }
-      if (best > 0.0f) {
-        self_c = 0.5f * cfg.self_weight * best;
-        const float4 si = rv.spheres[bi], sj = rv.spheres[bj];
-        const int ki = rv.sph_link[bi], kj = rv.sph_link[bj];
-        const V3 pi = xf_point(C + 12 * ki, si.x, si.y, si.z), pj = xf_point(C + 12 * kj, sj.x, sj.y, sj.z);
-        const V3 g = cfg.self_weight * (pj - pi);
-        chain_add(ki, pi, g, mk3(0, 0, 0));
-        chain_add(kj, pj, mk3(-g.x, -g.y, -g.z), mk3(0, 0, 0));
-      }
-    }
-    if (a.self_cost) a.self_cost[e] = self_c;
-    // ---- scene collision
-    float scene_c = 0.0f;
-    const int env = (a.env_query_idx != nullptr) ? __ldg(a.env_query_idx + b) : 0;
-    if (do_scene && rv.n_lp > 0) {
-      // link level first: which cuboids can a link's spheres touch at all?
-#pragma unroll 1
-      for (int ca = 0; ca < rv.n_cl; ++ca) {
-        const int k = rv.cl_link[ca];
-        const float *Tk = C + 12 * k;
-        unsigned cmask = 0u;
-        int ce = 0, ncub = 0;
-        if (SCENE & 1) {
-          ce = env < a.cuboids.num_envs ? env : 0;
-          ncub = a.cuboids.count[ce];
-          if (ncub > a.cuboids.max_n) ncub = a.cuboids.max_n;
-          const float4 cb = rv.cl_bound_scene[ca];
-          if (cb.w >= 0.0f) {
-            const V3 cw = xf_point(Tk, cb.x, cb.y, cb.z);
-            if (ncub > 32) {
-              cmask = 0xffffffffu;  // more cuboids than mask bits: no culling
-            } else {
-              for (int i = 0; i < ncub; ++i) {
-                const int kk = ce * a.cuboids.max_n + i;
-                if (a.cuboids.enable[kk] != 1) continue;
-                const ObsFrame f = load_obs_frame(a.cuboids.inv_pose + 8 * kk);
-                const SdfGrad sg = cuboid_sdf_grad(to_obstacle(f, cw), ldgf(a.cuboids.dims + 4 * kk), ldgf(a.cuboids.dims + 4 * kk + 1),
-                                                   ldgf(a.cuboids.dims + 4 * kk + 2));
-                if (sg.sdf < cb.w + cfg.scene_activation) cmask |= (1u << i);
-              }
-            }
-          }
-        }
-#pragma unroll 4
-        for (int s = rv.cl_start[ca]; s < rv.cl_start[ca + 1]; ++s) {
-          const float4 sp = rv.spheres[s];
-          float c = 0.0f;
-          V3 g = mk3(0, 0, 0);
-          V3 pw = mk3(0, 0, 0);
-          const bool need_pos = (a.robot_spheres != nullptr) || (sp.w >= 0.0f && (cmask != 0u || (SCENE & 2)));
-          if (need_pos) pw = xf_point(Tk, sp.x, sp.y, sp.z);
-          if (sp.w >= 0.0f) {
-            const float radj = sp.w + cfg.scene_activation;
-            if ((SCENE & 1) && cmask != 0u) {
-              for (int i = 0; i < ncub; ++i) {
-                if (ncub <= 32 && !((cmask >> i) & 1u)) continue;
-                const int kk = ce * a.cuboids.max_n + i;
-                if (a.cuboids.enable[kk] != 1) continue;
-                const ObsFrame f = load_obs_frame(a.cuboids.inv_pose + 8 * kk);
-                const SdfGrad sg = cuboid_sdf_grad(to_obstacle(f, pw), ldgf(a.cuboids.dims + 4 * kk), ldgf(a.cuboids.dims + 4 * kk + 1),
-                                                   ldgf(a.cuboids.dims + 4 * kk + 2));
-                const float pen = radj - sg.sdf;
-                if (pen > 0.0f) {
-                  float ac, as;
-                  collision_activation(pen, cfg.scene_activation, ac, as);
-                  c += cfg.scene_weight * ac;
-                  g = g + (cfg.scene_weight * as) * from_obstacle(f, sg.n);
-                }
-              }
-            }
-            if (SCENE & 2) {
-              CuboidSet none{};
-              c += sphere_scene_discrete<2>(pw, sp.w, cfg.scene_activation, cfg.scene_weight, none, a.voxels, env, g);
-            }
-          }
-          if (a.robot_spheres) reinterpret_cast<float4 *>(a.robot_spheres)[(size_t)e * S + s] = make_float4(pw.x, pw.y, pw.z, sp.w);
-          if (a.scene_cost) a.scene_cost[(size_t)e * S + s] = c;
-          scene_c += c;
-          if (g.x != 0.0f || g.y != 0.0f || g.z != 0.0f) chain_add(k, pw, g, mk3(0, 0, 0));
-        }
-      }
-    } else {
-#pragma unroll 1
-      for (int s = 0; s < S; ++s) {  // no link table (or no scene): plain loop over spheres
-        const float4 sp = rv.spheres[s];
-        const int k = rv.sph_link[s];
-        const V3 pw = xf_point(C + 12 * k, sp.x, sp.y, sp.z);
-        float c = 0.0f;
-        V3 g = mk3(0, 0, 0);
-        if (do_scene) c = sphere_scene_discrete<SCENE>(pw, sp.w, cfg.scene_activation, cfg.scene_weight, a.cuboids, a.voxels, env, g);
-        if (a.robot_spheres) reinterpret_cast<float4 *>(a.robot_spheres)[(size_t)e * S + s] = make_float4(pw.x, pw.y, pw.z, sp.w);
-        if (a.scene_cost) a.scene_cost[(size_t)e * S + s] = c;
-        scene_c += c;
-        if (g.x != 0.0f || g.y != 0.0f || g.z != 0.0f) chain_add(k, pw, g, mk3(0, 0, 0));
-      }
-    }
-    // ---- outputs
-#pragma unroll 1
-    for (int d = 0; d < D; ++d) a.grad_q[(size_t)e * D + d] = gqs[d * T];
-    a.cost[e] = cs_cost + pose_c + scene_c + self_c;
   }
 }
 
@@ -2522,6 +1869,124 @@ int persistent_grid(K kernel, int block, size_t smem, long long work_items) {
   if (g > work_items) g = work_items;
   if (g < 1) g = 1;
   return (int)g;
+}
+
+// Launch plan of a fused rollout kernel: its CTA shape for one robot geometry on one device.  The key holds everything the plan
+// depends on and is compared field by field.
+struct PlanKey {
+  const void *kernel;
+  int device;
+  size_t fixed_bytes;  // shared memory per CTA besides the rows: the staged robot blob, plus the trajectory kernels' halo
+  int unit_floats;     // shared floats per unit of work: a warp's row (or pair of rows), or a team's row
+  int horizon;         // trajectory and fused-dynamics kernels: waypoints per seed, which their scores use (0 elsewhere)
+  int nl, dof;         // fused-dynamics kernel: links and dofs, which size its dynamics tile (0 elsewhere)
+  bool operator==(const PlanKey &o) const {
+    return kernel == o.kernel && device == o.device && fixed_bytes == o.fixed_bytes && unit_floats == o.unit_floats &&
+           horizon == o.horizon && nl == o.nl && dof == o.dof;
+  }
+};
+struct Plan {
+  int nw = 0;       // warps per CTA; 0: no CTA of this kernel fits the geometry
+  int per_sm = 0;   // resident CTAs per SM (not queried for team kernels, which run one CTA per SM)
+  int R = 0;        // fused-dynamics kernel: rows per dynamics chunk
+  size_t smem = 0;  // dynamic shared memory per CTA
+};
+
+// Standard, arm, trajectory and big kernels: the warps per CTA (max_nw down to 1) that keep the most warps resident per SM --
+// shared memory is the limiter for big robots; ties go to the larger CTA so the blob is staged fewer times.
+Plan plan_warps(const PlanKey &k, size_t limit, int max_nw) {
+  Plan p;
+  double best = 0.0;
+  for (int nw = max_nw; nw >= 1; --nw) {
+    const size_t need = k.fixed_bytes + (size_t)nw * k.unit_floats * sizeof(float);
+    if (need > limit) continue;
+    int per_sm = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k.kernel, nw * 32, need) != cudaSuccess) continue;
+    double score = (double)per_sm * nw;
+    if (k.horizon > 0) {  // trajectory: rows of the last tile of a trajectory idle, and halo waypoints cost 2 extra FK per tile
+      const int tiles = (k.horizon + nw - 1) / nw;
+      score *= (double)k.horizon / ((double)tiles * nw + 0.3 * 2.0 * (tiles - 1));
+    }
+    if (score > best) {
+      best = score;
+      p = Plan{nw, per_sm, 0, need};
+    }
+  }
+  return p;
+}
+
+// Team kernels: the largest multiple of the team size, up to kBigWarps warps, whose teams fit.  No occupancy query: the grid is
+// one CTA per SM.
+Plan plan_team(const PlanKey &k, size_t limit, int team) {
+  for (int w = kBigWarps; w >= team; w -= team) {
+    const size_t need = k.fixed_bytes + (size_t)(w / team) * k.unit_floats * sizeof(float);
+    if (need <= limit) return Plan{w, 0, 0, need};
+  }
+  return Plan{};
+}
+
+// Fused-dynamics kernel: (warps per CTA, rows per dynamics chunk) that keeps the most warps resident; R is a multiple of the warp
+// count so a chunk is a whole number of waypoint tiles.
+Plan plan_dyn(const PlanKey &k, size_t limit) {
+  Plan p;
+  double best = 0.0;
+  for (int nw = kWarpsPerCta; nw >= 1; nw >>= 1) {
+    for (int R = 32; R >= 8 && R >= nw; R >>= 1) {
+      const size_t need = k.fixed_bytes + (size_t)nw * k.unit_floats * sizeof(float) +
+                          (size_t)dyn::tile_floats(k.nl, k.dof, R) * sizeof(float);
+      if (need > limit) continue;
+      int per_sm = 0;
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k.kernel, nw * 32, need) != cudaSuccess || per_sm < 1) continue;
+      // resident warps, discounted for idle rows of the last tile / chunk of a trajectory and for short dynamics chunks
+      // (the recursion's serial depth is paid once per chunk whatever its width)
+      const int chunks = (k.horizon + R - 1) / R;
+      const double score = (double)per_sm * nw * ((double)k.horizon / ((double)chunks * R)) * (0.75 + 0.25 * R / 32.0);
+      if (score > best) {
+        best = score;
+        p = Plan{nw, per_sm, R, need};
+      }
+    }
+  }
+  return p;
+}
+
+// This thread's plans, replaced round-robin.
+struct PlanEntry {
+  PlanKey key;
+  Plan plan;
+};
+constexpr int kPlanSlots = 16;
+thread_local PlanEntry g_plans[kPlanSlots];
+thread_local int g_plans_used = 0, g_plans_next = 0;
+
+// The plan of key k: cached, or made by make(k, limit).  Before planning, the kernel's dynamic shared-memory cap (a device-wide
+// setting) is set to the opt-in limit less the kernel's static shared memory.  That value depends only on (kernel, device), so
+// no thread planning another geometry can lower it under a plan this thread cached.
+template <typename F>
+cudaError_t cached_plan(const PlanKey &k, const DevInfo &d, F make, Plan &out) {
+  for (int i = 0; i < g_plans_used; ++i) {
+    if (g_plans[i].key == k) {
+      out = g_plans[i].plan;
+      return cudaSuccess;
+    }
+  }
+  cudaFuncAttributes fa;
+  cudaError_t e = cudaFuncGetAttributes(&fa, k.kernel);
+  if (e != cudaSuccess) return e;
+  const size_t limit = (size_t)d.max_smem - fa.sharedSizeBytes;
+  e = cudaFuncSetAttribute(k.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit);
+  if (e != cudaSuccess) return e;
+  out = make(k, limit);
+  g_plans[g_plans_next] = PlanEntry{k, out};
+  g_plans_next = (g_plans_next + 1) % kPlanSlots;
+  if (g_plans_used < kPlanSlots) ++g_plans_used;
+  return cudaSuccess;
+}
+
+// A per-call override from the environment (tests switch these inside one process); dflt when unset.
+int env_int(const char *name, int dflt) {
+  const char *s = getenv(name);
+  return s ? atoi(s) : dflt;
 }
 
 inline CuboidSet to_dev(const cb200_cuboid_set *c) {
@@ -3207,11 +2672,6 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
   }
   a.blob_smem_bytes = h.smem_bytes;
   a.eval_floats = eval_smem_floats(h.nl, h.D, h.S, h.L, h.n_cl);
-  static const int phase_sync_env = []() {
-    const char *e = getenv("CB200_PHASE_SYNC");
-    return e ? atoi(e) : 0;
-  }();
-  a.phase_sync = phase_sync_env;
   const bool expand = sp != nullptr && sp->out_position != nullptr && sp->out_velocity != nullptr &&
                       sp->out_acceleration != nullptr && sp->out_jerk != nullptr && sp->out_dt != nullptr;
   // mesh obstacles: scene bit 2.  The in-kernel spline schedule and the fused-dynamics kernel have no mesh build; they refuse mesh
@@ -3247,7 +2707,8 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
   }
   DevInfo &d = dev_info();
   const bool traj = cfg->use_sweep != 0;
-  if (traj && cfg->use_speed_metric && a.dt == nullptr && a.spl.knots == nullptr) return ret(cudaErrorInvalidValue);
+  const bool spline = a.spl.knots != nullptr;  // B-spline front end: rows are evaluated from the knots inside the kernel
+  if (traj && cfg->use_speed_metric && a.dt == nullptr && !spline) return ret(cudaErrorInvalidValue);
   // the adjoint of the spline front end runs right behind the rollout kernel on the same stream
   auto finish = [&]() -> int {
     const int rc = launch_status();
@@ -3257,208 +2718,71 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
                                                    io->horizon, h.D, sp->n_knots, sp->degree, stream));
   };
   // kernels are specialised on the obstacle types present (bit 0 cuboids, bit 1 voxel grids) so that e.g. the
-  // IK kernel carries no ESDF code: the fused kernel's instruction footprint is what limits it.
+  // IK kernel carries no ESDF code: the fused kernel's instruction footprint is what limits it.  Mesh scenes take one build per
+  // kernel family, SCENE = 7, which checks at run time whether cuboids and ESDF grids are present.
   const int scene = (cfg->scene_weight > 0.0f ? ((a.cuboids.inv_pose ? 1 : 0) | (a.voxels.inv_pose ? 2 : 0)) : 0);
-  // Mesh scenes take one build per kernel family, SCENE = 7, which checks at run time whether cuboids and ESDF grids are
-  // present (5 kernels instead of 20 for SCENE in 4..7).  Cached launch plans of mesh scenes use slot 4.
-  const int sidx = mesh ? 4 : scene;
+  // arms (few links / spheres): the row state is ~3 KB, so residency is register-bound; their 80-register builds keep 24 instead
+  // of 16 warps per SM resident and are ~7 % faster on the IK workload (slower for humanoids, where shared memory bounds
+  // residency anyway)
+  const bool arm_sized = h.nl <= 24 && h.S <= 128;
+  // CB200_QUEUE = 0: static striding even when the caller gives a ticket counter
+  int32_t *const counter = env_int("CB200_QUEUE", 1) != 0 ? io->work_counter : nullptr;
   using KernelT = void (*)(const FusedArgs);
-  static KernelT const table[5][4] = {
-      {rollout_fused_kernel<0, false>, rollout_fused_kernel<1, false>, rollout_fused_kernel<2, false>, rollout_fused_kernel<3, false>},
-      {rollout_traj_kernel<0, false>, rollout_traj_kernel<1, false>, rollout_traj_kernel<2, false>, rollout_traj_kernel<3, false>},
-      {rollout_tile_kernel<0>, rollout_tile_kernel<1>, rollout_tile_kernel<2>, rollout_tile_kernel<3>},
-      // B-spline front end: rows are evaluated from the knots inside the kernel
-      {rollout_fused_kernel<0, true>, rollout_fused_kernel<1, true>, rollout_fused_kernel<2, true>, rollout_fused_kernel<3, true>},
-      {rollout_traj_kernel<0, true>, rollout_traj_kernel<1, true>, rollout_traj_kernel<2, true>, rollout_traj_kernel<3, true>}};
-  // arms (few links / spheres): the row state is ~3 KB, so residency is register-bound; an 80-register build keeps
-  // 24 instead of 16 warps per SM resident and is ~7 % faster on the IK workload (slower for humanoids, where shared
-  // memory bounds residency anyway).  CB200_ARM_REGCAP=0 disables.
-  static KernelT const arm_table[4] = {rollout_fused_kernel<0, false, 3>, rollout_fused_kernel<1, false, 3>,
-                                       rollout_fused_kernel<2, false, 3>, rollout_fused_kernel<3, false, 3>};
-  static const int arm_regcap = []() {
-    const char *e = getenv("CB200_ARM_REGCAP");
-    return e ? atoi(e) : 1;
-  }();
-  static const int arm_esdf = []() {  // 0: arms against an ESDF always take the big-robot kernel (the round-2 default before 3l)
-    const char *e = getenv("CB200_ARM_ESDF");
-    return e ? atoi(e) : 1;
-  }();
-  // small robots (arms) in discrete mode: thread-per-row "lane" schedule
-  static const int lane_env = []() {
-    const char *e = getenv("CB200_LANE");
-    return e ? atoi(e) : 0;  // off by default: measured slower than warp-per-row
-  }();
-  if (!traj && lane_env != 0 && !mesh && h.nl <= 24 && h.S <= 128 && a.spl.knots == nullptr && a.sphere_cfgs == nullptr) {
-    static KernelT const lane_table[4] = {rollout_lane_kernel<0>, rollout_lane_kernel<1>, rollout_lane_kernel<2>,
-                                          rollout_lane_kernel<3>};
-    const LaneLayout ll = lane_layout(h.smem_bytes, kLaneThreads, h.nl, h.D, h.n_cl);
-    KernelT lk = lane_table[scene];
-    static thread_local size_t lane_cfg[4] = {0, 0, 0, 0};
-    static thread_local int lane_per_sm[4] = {0, 0, 0, 0};
-    const size_t lane_key = ll.total_bytes ^ ((size_t)(d.ordinal + 1) << 48);
-    if (lane_cfg[scene] != lane_key) {
-      int per_sm = 0;
-      if (cudaFuncSetAttribute(lk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ll.total_bytes) == cudaSuccess)
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lk, kLaneThreads, ll.total_bytes);
-      else
-        (void)cudaGetLastError();
-      lane_per_sm[scene] = per_sm;
-      lane_cfg[scene] = lane_key;
-    }
-    if (lane_per_sm[scene] >= 2) {
-      const long long need = (N + kLaneThreads - 1) / kLaneThreads;
-      long long g = (long long)d.sm_count * lane_per_sm[scene];
-      if (g > need) g = need;
-      g_last_variant = CB200_VARIANT_LANE;
-      CB200_LAUNCH(lk, (int)g, kLaneThreads, ll.total_bytes, (cudaStream_t)stream, a);
-      return launch_status();
-    }
-  }
-  // tile schedule (kept for A/B; off by default: measured slower than the warp-per-row kernel)
-  static const int tile_env = []() {
-    const char *e = getenv("CB200_TILE");
-    return e ? atoi(e) : 0;
-  }();
-  if (!traj && tile_env != 0 && !mesh && a.spl.knots == nullptr && a.sphere_cfgs == nullptr) {
-    const TileLayout tl = tile_layout(h.smem_bytes, kWarpsPerCta, h.nl, h.D, h.S, h.L, h.n_cl);
-    KernelT tk = table[2][scene];
-    static thread_local size_t tile_cfg[4] = {0, 0, 0, 0};
-    static thread_local int tile_per_sm[4] = {0, 0, 0, 0};
-    cudaFuncAttributes fa;
-    const size_t tile_key = tl.total_bytes ^ ((size_t)(d.ordinal + 1) << 48);
-    if (tile_cfg[scene] != tile_key) {
-      if (cudaFuncGetAttributes(&fa, tk) == cudaSuccess && 2 * (tl.total_bytes + fa.sharedSizeBytes + 1024) <= (size_t)d.max_smem + 4096 &&
-          cudaFuncSetAttribute(tk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tl.total_bytes) == cudaSuccess) {
-        int per_sm = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, tk, kWarpsPerCta * 32, tl.total_bytes);
-        tile_per_sm[scene] = per_sm;
-      } else {
-        tile_per_sm[scene] = 0;
-        (void)cudaGetLastError();
-      }
-      tile_cfg[scene] = tile_key;
-    }
-    if (tile_per_sm[scene] >= 2) {
-      const long long n_tiles = (N + tl.T - 1) / tl.T;
-      long long g = (long long)d.sm_count * tile_per_sm[scene];
-      if (g > n_tiles) g = n_tiles;
-      g_last_variant = CB200_VARIANT_TILE;
-      CB200_LAUNCH(tk, (int)g, kWarpsPerCta * 32, tl.total_bytes, (cudaStream_t)stream, a);
-      return launch_status();
-    }
-  }
+  Plan p;
   // big robots (humanoids) and ESDF scenes, discrete mode: the list-based kernel with up to 16 warps per SM (see
   // rollout_fused_big_kernel).  CB200_BIG = 0 / 1 forces it off / on.  Default: on when a row of the standard layout exceeds
-  // 8 KB, and against an ESDF for robots that have no 80-register arm build (or too few rows to fill it: see arm_sized below).
-  const char *big_str = getenv("CB200_BIG");  // read per call: tests switch it inside one process
-  const int big_env = big_str ? atoi(big_str) : -1;
-  const bool big_fit = !traj && a.spl.knots == nullptr && h.n_lp > 0 && h.P > 0;
+  // 8 KB, and against an ESDF for robots that have no 80-register arm build (or too few rows to fill it).
   // (arms against an ESDF: the 80-register arm build of the standard kernel is faster at full batches -- Franka + 256^3 ESDF,
   //  16,384 rows: 0.0793 vs 0.0864 ms -- so they come here only when rows are scarce enough for two warps per row)
-  const bool arm_sized = arm_regcap != 0 && arm_esdf != 0 && h.nl <= 24 && h.S <= 128;
+  const int big_env = env_int("CB200_BIG", -1);
+  const bool big_fit = !traj && !spline && h.n_lp > 0 && h.P > 0;
   const bool big_want = big_env >= 0 ? big_env != 0
                                      : ((size_t)a.eval_floats * sizeof(float) > 8192 ||
                                         ((scene & 2) != 0 && (!arm_sized || N * 2 <= (long long)d.sm_count * kBigWarps)));
   if (big_fit && big_want) {
-    static KernelT const big_table[2][4] = {
-        {rollout_fused_big_kernel<0>, rollout_fused_big_kernel<1>, rollout_fused_big_kernel<2>, rollout_fused_big_kernel<3>},
-        {rollout_fused_big_kernel<0, true>, rollout_fused_big_kernel<1, true>, rollout_fused_big_kernel<2, true>,
-         rollout_fused_big_kernel<3, true>}};
-    static KernelT const big_mesh[2] = {rollout_fused_big_kernel<7>, rollout_fused_big_kernel<7, true>};
-    const int small_arm = (h.nl <= 24 && h.S <= 128) ? 1 : 0;
+    static KernelT const big[4] = {rollout_fused_big_kernel<0>, rollout_fused_big_kernel<1>, rollout_fused_big_kernel<2>,
+                                   rollout_fused_big_kernel<3>};
+    static KernelT const big_arm[4] = {rollout_fused_big_kernel<0, true>, rollout_fused_big_kernel<1, true>,
+                                       rollout_fused_big_kernel<2, true>, rollout_fused_big_kernel<3, true>};
     // (an 18-warp build -- 576 threads, 96 registers, small spills -- measured 0.237 ms on G1-29 against 0.219 ms for 16 warps)
-    const int maxw = kBigWarps;
-    KernelT bk = mesh ? big_mesh[small_arm] : big_table[small_arm][scene];
-    struct BigPlan {
-      long long key = -1;
-      int nw = 0, per_sm = 0;
-    };
-    static thread_local BigPlan bplans[2][5];
-    BigPlan &bp = bplans[small_arm][sidx];
+    KernelT bk = arm_sized ? (mesh ? rollout_fused_big_kernel<7, true> : big_arm[scene])
+                           : (mesh ? rollout_fused_big_kernel<7> : big[scene]);
     const int big_floats = big_smem_floats(h.nl, h.D, h.S, h.L, h.n_cl);
-    const long long bkey = ((long long)h.smem_bytes << 32) ^ ((long long)big_floats << 8) ^ ((long long)(d.ordinal + 1) << 56);
-    if (bkey != bp.key) {
-      cudaFuncAttributes fa;
-      cudaError_t e0 = cudaFuncGetAttributes(&fa, bk);
-      if (e0 != cudaSuccess) return ret(e0);
-      const size_t limit = (size_t)d.max_smem - fa.sharedSizeBytes;
-      cudaError_t e1 = cudaFuncSetAttribute(bk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit);
-      if (e1 != cudaSuccess) return ret(e1);
-      static const int force_nw = []() {
-        const char *e = getenv("CB200_FORCE_NW");
-        return e ? atoi(e) : 0;
-      }();
-      int best = 0;
-      BigPlan cand;
-      for (int nw = maxw; nw >= 1; --nw) {
-        if (force_nw > 0 && nw != force_nw) continue;
-        const size_t need = (size_t)h.smem_bytes + (size_t)nw * big_floats * sizeof(float);
-        if (need > limit) continue;
-        int per_sm = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bk, nw * 32, need) != cudaSuccess || per_sm < 1) continue;
-        if (per_sm * nw > best) {
-          best = per_sm * nw;
-          cand.nw = nw, cand.per_sm = per_sm;
-        }
-      }
-      if (cand.nw > 0) {
-        cand.key = bkey;
-        bp = cand;
-      }
-    }
+    Plan bp;
+    cudaError_t e = cached_plan(PlanKey{(const void *)bk, d.ordinal, (size_t)h.smem_bytes, big_floats, 0, 0, 0}, d,
+                                [](const PlanKey &k, size_t limit) { return plan_warps(k, limit, kBigWarps); }, bp);
+    if (e != cudaSuccess) return ret(e);
     // Small batches: a team of warps per row (rollout_fused_team_kernel) when the rows would leave at least half of the
     // resident warp slots idle.  CB200_TEAM = 0 / 2 / 4 forces the team size.  The team kernel has no mesh build: mesh scenes
     // stay on the big kernel.
-    if (!mesh) {
-      const char *ts = getenv("CB200_TEAM");
-      const int team_env = ts ? atoi(ts) : -1;
-      const long long slots = (long long)d.sm_count * maxw;
+    if (!mesh && h.nl <= 64) {
+      const int team_env = env_int("CB200_TEAM", -1);
+      const long long slots = (long long)d.sm_count * kBigWarps;
       // Measured rule.  Small robots (row <= 8 KB, here because of the ESDF): two warps per
       // row while that leaves warp slots free.  Humanoids: four warps per row while that leaves slots free, then two -- always
       // when the one-warp plan is shared-memory limited (G1-43: 11 rows per SM; 8 teams of 2 warps are 16 warps
       // at 8,192 rows), otherwise (G1-29) up to about two rows per warp slot.
       const bool small_robot = (size_t)a.eval_floats * sizeof(float) <= 8192;
-      const bool smem_limited = bp.key == bkey && bp.nw * bp.per_sm < maxw;
+      const bool smem_limited = bp.nw > 0 && bp.nw * bp.per_sm < kBigWarps;
       int team = 0;
       if (team_env >= 0) team = team_env;
       else if (small_robot) team = (N * 2 <= slots) ? 2 : 0;
       else if (N * 4 <= slots) team = 4;
       else if (smem_limited || N <= 2 * slots) team = 2;
-      if ((team == 2 || team == 4) && h.nl <= 64) {
-        static KernelT const team_table[2][4] = {
-            {rollout_fused_team_kernel<0, 2>, rollout_fused_team_kernel<1, 2>, rollout_fused_team_kernel<2, 2>,
-             rollout_fused_team_kernel<3, 2>},
-            {rollout_fused_team_kernel<0, 4>, rollout_fused_team_kernel<1, 4>, rollout_fused_team_kernel<2, 4>,
-             rollout_fused_team_kernel<3, 4>}};
-        KernelT tk = team_table[team == 4][scene];
+      if (team == 2 || team == 4) {
+        static KernelT const team2[4] = {rollout_fused_team_kernel<0, 2>, rollout_fused_team_kernel<1, 2>,
+                                         rollout_fused_team_kernel<2, 2>, rollout_fused_team_kernel<3, 2>};
+        static KernelT const team4[4] = {rollout_fused_team_kernel<0, 4>, rollout_fused_team_kernel<1, 4>,
+                                         rollout_fused_team_kernel<2, 4>, rollout_fused_team_kernel<3, 4>};
+        KernelT tk = team == 4 ? team4[scene] : team2[scene];
         const int team_floats = (big_floats + team_extra_floats(team, h.nl) + 3) & ~3;
-        static thread_local long long tkeys[2][4] = {{-1, -1, -1, -1}, {-1, -1, -1, -1}};
-        static thread_local int tnw[2][4];
-        long long &tkey = tkeys[team == 4][scene];
-        if (tkey != bkey) {
-          cudaFuncAttributes fa;
-          cudaError_t e0 = cudaFuncGetAttributes(&fa, tk);
-          if (e0 != cudaSuccess) return ret(e0);
-          const size_t limit = (size_t)d.max_smem - fa.sharedSizeBytes;
-          cudaError_t e1 = cudaFuncSetAttribute(tk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit);
-          if (e1 != cudaSuccess) return ret(e1);
-          int nw = 0;
-          for (int w = maxw; w >= team; w -= team) {
-            if ((size_t)h.smem_bytes + (size_t)(w / team) * team_floats * sizeof(float) <= limit) {
-              nw = w;
-              break;
-            }
-          }
-          tnw[team == 4][scene] = nw;
-          tkey = bkey;
-        }
-        const int nw = tnw[team == 4][scene];
-        if (nw >= team) {
+        e = cached_plan(PlanKey{(const void *)tk, d.ordinal, (size_t)h.smem_bytes, team_floats, 0, 0, 0}, d,
+                        [team](const PlanKey &k, size_t limit) { return plan_team(k, limit, team); }, p);
+        if (e != cudaSuccess) return ret(e);
+        if (p.nw > 0) {
           a.eval_floats = team_floats;
-          const char *qs = getenv("CB200_QUEUE");
-          a.work_counter = (qs && atoi(qs) == 0) ? nullptr : io->work_counter;
-          const int nteams = nw / team;
-          const size_t smem_b = (size_t)h.smem_bytes + (size_t)nteams * team_floats * sizeof(float);
+          a.work_counter = counter;
+          const int nteams = p.nw / team;
           long long g = d.sm_count;
           const long long need_ctas = (N + nteams - 1) / nteams;
           // spread the rows over all SMs first: fewer teams per CTA rather than fewer CTAs
@@ -3470,181 +2794,103 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
           long long ctas = (N + launch_teams - 1) / launch_teams;
           if (ctas > g) ctas = g;
           g_last_variant = team == 4 ? CB200_VARIANT_TEAM4 : CB200_VARIANT_TEAM2;
-          CB200_LAUNCH(tk, (int)(ctas < 1 ? 1 : ctas), launch_teams * team * 32, smem_b, (cudaStream_t)stream, a);
+          CB200_LAUNCH(tk, (int)(ctas < 1 ? 1 : ctas), launch_teams * team * 32, p.smem, (cudaStream_t)stream, a);
           return finish();
         }
       }
     }
-    if (bp.key == bkey) {
+    if (bp.nw > 0) {  // (no plan: the standard kernel below)
       a.eval_floats = big_floats;
-      {
-        const char *qs = getenv("CB200_QUEUE");
-        a.work_counter = (qs && atoi(qs) == 0) ? nullptr : io->work_counter;
-      }
-      const size_t smem_b = (size_t)h.smem_bytes + (size_t)bp.nw * big_floats * sizeof(float);
+      a.work_counter = counter;
       long long g = (long long)d.sm_count * bp.per_sm;
       const long long need_ctas = (N + bp.nw - 1) / bp.nw;
       if (g > need_ctas) g = need_ctas;
       g_last_variant = CB200_VARIANT_BIG;
-      CB200_LAUNCH(bk, (int)(g < 1 ? 1 : g), bp.nw * 32, smem_b, (cudaStream_t)stream, a);
+      CB200_LAUNCH(bk, (int)(g < 1 ? 1 : g), bp.nw * 32, bp.smem, (cudaStream_t)stream, a);
       return finish();
     }
   }
-  int variant = (traj ? 1 : 0) + (a.spl.knots != nullptr ? 3 : 0);
-  static KernelT const mesh_table[2] = {rollout_fused_kernel<7, false>, rollout_traj_kernel<7, false>};  // (variant 0 / 1)
-  KernelT kern = mesh ? mesh_table[variant] : table[variant][scene];
-  if (traj && h.nl <= 24 && h.S <= 128) {
-    static KernelT const traj_small[2][4] = {
-        {rollout_traj_kernel<0, false, true>, rollout_traj_kernel<1, false, true>, rollout_traj_kernel<2, false, true>,
-         rollout_traj_kernel<3, false, true>},
-        {rollout_traj_kernel<0, true, true>, rollout_traj_kernel<1, true, true>, rollout_traj_kernel<2, true, true>,
-         rollout_traj_kernel<3, true, true>}};
-    kern = mesh ? rollout_traj_kernel<7, false, true> : traj_small[a.spl.knots != nullptr ? 1 : 0][scene];
-  }
+  const size_t halo_bytes = traj ? (size_t)2 * h.S * sizeof(float4) : 0;
   if (io->dynamics != nullptr) {
     // inverse dynamics inside the trajectory kernel: rows must come from caller-provided states (or the expanded spline
     // schedule, which arrives here with a.spl.knots == nullptr) and the STATE c-space cost must be on
     const cb200_dynamics_params *dp = io->dynamics;
     if (dp->link_masses_com == nullptr || dp->link_inertias == nullptr || dp->gravity == nullptr || !traj ||
-        cfg->cspace_type != 2 || a.spl.knots != nullptr || a.vel == nullptr || a.acc == nullptr)
+        cfg->cspace_type != 2 || spline || a.vel == nullptr || a.acc == nullptr)
       return ret(cudaErrorInvalidValue);
     a.dyn = FusedArgs::Dyn{dp->link_masses_com, dp->link_inertias, dp->gravity};
-    // chunked kernel: (warps per CTA, rows per dynamics chunk) that keeps the most warps resident; R is a multiple of the warp
-    // count so a chunk is a whole number of waypoint tiles.  Cached per (scene variant, geometry, horizon, device).
     using DynKernelT = void (*)(const FusedArgs, const int);
-    static DynKernelT const dyn_table[4] = {rollout_traj_dyn_kernel<0>, rollout_traj_dyn_kernel<1>, rollout_traj_dyn_kernel<2>,
-                                            rollout_traj_dyn_kernel<3>};
-    DynKernelT dk = dyn_table[scene];
-    struct DynPlan {
-      long long key = -1;
-      int nw = 0, R = 0, per_sm = 0;
-      size_t smem = 0;
-    };
-    static thread_local DynPlan dplans[4];
-    DynPlan &dpl = dplans[scene];
-    const size_t halo = (size_t)2 * h.S * sizeof(float4);
-    const long long dkey = ((long long)h.smem_bytes << 32) ^ ((long long)a.eval_floats << 8) ^ ((long long)io->horizon << 40) ^
-                           ((long long)(d.ordinal + 1) << 56);
-    if (dkey != dpl.key) {
-      cudaFuncAttributes fa;
-      cudaError_t e0 = cudaFuncGetAttributes(&fa, dk);
-      if (e0 != cudaSuccess) return ret(e0);
-      const size_t limit = (size_t)d.max_smem - fa.sharedSizeBytes;
-      cudaError_t e1 = cudaFuncSetAttribute(dk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit);
-      if (e1 != cudaSuccess) return ret(e1);
-      double best = 0.0;
-      DynPlan cand;
-      for (int nw = kWarpsPerCta; nw >= 1; nw >>= 1) {
-        for (int R = 32; R >= 8 && R >= nw; R >>= 1) {
-          const size_t need = (size_t)h.smem_bytes + halo + (size_t)nw * a.eval_floats * sizeof(float) +
-                              (size_t)dyn::tile_floats(h.nl, h.D, R) * sizeof(float);
-          if (need > limit) continue;
-          int per_sm = 0;
-          if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, dk, nw * 32, need) != cudaSuccess || per_sm < 1) continue;
-          // resident warps, discounted for idle rows of the last tile / chunk of a trajectory and for short dynamics chunks
-          // (the recursion's serial depth is paid once per chunk whatever its width)
-          const int chunks = (io->horizon + R - 1) / R;
-          double score = (double)per_sm * nw * ((double)io->horizon / ((double)chunks * R)) * (0.75 + 0.25 * R / 32.0);
-          if (score > best) {
-            best = score;
-            cand.nw = nw, cand.R = R, cand.per_sm = per_sm, cand.smem = need;
-          }
-        }
-      }
-      if (cand.nw == 0) return ret(cudaErrorInvalidConfiguration);
-      cand.key = dkey;
-      dpl = cand;
-    }
-    long long grid_ll = (long long)d.sm_count * dpl.per_sm;
-    const long long need_ctas = (long long)io->batch_size * ((io->horizon + dpl.R - 1) / dpl.R);
+    static DynKernelT const traj_dyn[4] = {rollout_traj_dyn_kernel<0>, rollout_traj_dyn_kernel<1>, rollout_traj_dyn_kernel<2>,
+                                           rollout_traj_dyn_kernel<3>};
+    DynKernelT dk = traj_dyn[scene];
+    const cudaError_t e = cached_plan(PlanKey{(const void *)dk, d.ordinal, (size_t)h.smem_bytes + halo_bytes, a.eval_floats,
+                                              io->horizon, h.nl, h.D},
+                                      d, plan_dyn, p);
+    if (e != cudaSuccess) return ret(e);
+    if (p.nw == 0) return ret(cudaErrorInvalidConfiguration);
+    long long grid_ll = (long long)d.sm_count * p.per_sm;
+    const long long need_ctas = (long long)io->batch_size * ((io->horizon + p.R - 1) / p.R);
     if (grid_ll > need_ctas) grid_ll = need_ctas;
     g_last_variant = CB200_VARIANT_TRAJ_DYN;
-    CB200_LAUNCH(dk, (int)(grid_ll < 1 ? 1 : grid_ll), dpl.nw * 32, dpl.smem, (cudaStream_t)stream, a, dpl.R);
+    CB200_LAUNCH(dk, (int)(grid_ll < 1 ? 1 : grid_ll), p.nw * 32, p.smem, (cudaStream_t)stream, a, p.R);
     return finish();
   }
-  // rows per warp: 2 for arms of <= 16 links (one link per lane of a half-warp in the sparse J^T) from 1.5 rows per resident warp
-  // slot of the arm build (MINB CTAs of kWarpsPerCta warps per SM) up; with fewer rows a warp per row is faster (Franka + cuboids,
-  // H100 SXM at 400 W: 0.0183 vs 0.0255 ms at 1.0 rows per slot, 0.0274 vs 0.0270 ms at 1.5, 0.0324 vs 0.0271 ms at 2.0).  Not
-  // against an ESDF: that build spills (140 B) and measured 2 % slower (franka_16384_esdf).  CB200_ARM_PAIRS = 0 / 1 forces one /
-  // two rows per warp.
-  // Mesh scenes of arms stay on the 128-register build, one row per warp: an 80-register mesh build spilled 172 B (DESIGN.md
-  // section 4), so none is built.
+  // standard, arm and trajectory kernels: one warp per row (per pair of rows in the arms' paired build, per waypoint of a
+  // trajectory tile)
+  KernelT kern;
   int rows_per_warp = 1;
-  if (variant == 0 && !mesh && arm_regcap != 0 && (scene <= 1 || arm_esdf != 0) && h.nl <= 24 && h.S <= 128) {
-    const char *ps = getenv("CB200_ARM_PAIRS");  // read per call: tests switch it inside one process
-    const int pairs_env = ps ? atoi(ps) : -1;
+  bool arm = false;
+  if (traj) {
+    static KernelT const traj_full[2][4] = {
+        {rollout_traj_kernel<0, false>, rollout_traj_kernel<1, false>, rollout_traj_kernel<2, false>, rollout_traj_kernel<3, false>},
+        {rollout_traj_kernel<0, true>, rollout_traj_kernel<1, true>, rollout_traj_kernel<2, true>, rollout_traj_kernel<3, true>}};
+    static KernelT const traj_small[2][4] = {
+        {rollout_traj_kernel<0, false, true>, rollout_traj_kernel<1, false, true>, rollout_traj_kernel<2, false, true>,
+         rollout_traj_kernel<3, false, true>},
+        {rollout_traj_kernel<0, true, true>, rollout_traj_kernel<1, true, true>, rollout_traj_kernel<2, true, true>,
+         rollout_traj_kernel<3, true, true>}};
+    if (arm_sized) kern = mesh ? rollout_traj_kernel<7, false, true> : traj_small[spline][scene];
+    else kern = mesh ? rollout_traj_kernel<7, false> : traj_full[spline][scene];
+  } else if (!spline && !mesh && arm_sized) {
+    // rows per warp: 2 for arms of <= 16 links (one link per lane of a half-warp in the sparse J^T) from 1.5 rows per resident
+    // warp slot of the arm build (3 CTAs of kWarpsPerCta warps per SM) up; with fewer rows a warp per row is faster (Franka +
+    // cuboids, H100 SXM at 400 W: 0.0183 vs 0.0255 ms at 1.0 rows per slot, 0.0274 vs 0.0270 ms at 1.5, 0.0324 vs 0.0271 ms at
+    // 2.0).  Not against an ESDF: that build spills (140 B) and measured 2 % slower (franka_16384_esdf).  CB200_ARM_PAIRS = 0 / 1
+    // forces one / two rows per warp.
+    // Mesh scenes of arms stay on the 128-register build, one row per warp: an 80-register mesh build spilled 172 B (DESIGN.md
+    // section 4), so none is built.
+    static KernelT const arm_rows[4] = {rollout_fused_kernel<0, false, 3>, rollout_fused_kernel<1, false, 3>,
+                                        rollout_fused_kernel<2, false, 3>, rollout_fused_kernel<3, false, 3>};
+    static KernelT const arm_pairs[2] = {rollout_fused_kernel<0, false, 3, 2>, rollout_fused_kernel<1, false, 3, 2>};
+    const int pairs_env = env_int("CB200_ARM_PAIRS", -1);
     const bool pairs = h.nl <= 16 && (scene & 2) == 0 &&
                        (pairs_env >= 0 ? pairs_env != 0 : 2LL * N >= 3LL * d.sm_count * 3 * kWarpsPerCta);
-    static KernelT const arm_pairs_table[2] = {rollout_fused_kernel<0, false, 3, 2>, rollout_fused_kernel<1, false, 3, 2>};
-    kern = pairs ? arm_pairs_table[scene] : arm_table[scene];
+    kern = pairs ? arm_pairs[scene] : arm_rows[scene];
     rows_per_warp = pairs ? 2 : 1;
-    variant = pairs ? 6 : 5;
+    arm = true;
+  } else {
+    static KernelT const fused[2][4] = {
+        {rollout_fused_kernel<0, false>, rollout_fused_kernel<1, false>, rollout_fused_kernel<2, false>, rollout_fused_kernel<3, false>},
+        {rollout_fused_kernel<0, true>, rollout_fused_kernel<1, true>, rollout_fused_kernel<2, true>, rollout_fused_kernel<3, true>}};
+    kern = mesh ? rollout_fused_kernel<7, false> : fused[spline][scene];
   }
-  const int warp_floats = rows_per_warp * a.eval_floats;
-  const int minb = sidx;  // part of the plan-cache key
-  // warps per CTA: the count that keeps the most warps resident per SM (shared memory is the limiter for
-  // big robots); ties go to the larger CTA so the blob is staged fewer times.  Cached per (kernel, geometry).
-  struct Plan {
-    long long key = -1;
-    int nw = 0, per_sm = 0;
-  };
-  static thread_local Plan plans[7][5];
-  Plan &pl = plans[variant][sidx];
-  const size_t halo_bytes = traj ? (size_t)2 * h.S * sizeof(float4) : 0;
-  const long long key = ((long long)h.smem_bytes << 32) ^ ((long long)warp_floats << 8) ^ (long long)minb ^
-                        (traj ? ((long long)io->horizon << 40) : 0) ^ ((long long)(d.ordinal + 1) << 56);
-  if (key != pl.key) {
-    cudaFuncAttributes fa;
-    cudaError_t e0 = cudaFuncGetAttributes(&fa, kern);
-    if (e0 != cudaSuccess) return ret(e0);
-    const size_t limit = (size_t)d.max_smem - fa.sharedSizeBytes;  // opt-in limit covers static + dynamic
-    const size_t max_need = (size_t)h.smem_bytes + halo_bytes + (size_t)kWarpsPerCta * warp_floats * sizeof(float);
-    const size_t cap = std::min(max_need, limit);
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cap);
-    if (e != cudaSuccess) return ret(e);
-    int best_nw = 0, best_per_sm = 0;
-    double best_score = 0.0;
-    static const int force_nw = []() {  // tuning knob: pin the warps per CTA (0 = choose by residency)
-      const char *e = getenv("CB200_FORCE_NW");
-      return e ? atoi(e) : 0;
-    }();
-    for (int nw = kWarpsPerCta; nw >= 1; --nw) {
-      if (force_nw > 0 && nw != force_nw) continue;
-      const size_t need = (size_t)h.smem_bytes + halo_bytes + (size_t)nw * warp_floats * sizeof(float);
-      if (need > limit) continue;
-      int per_sm = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, nw * 32, need) != cudaSuccess) continue;
-      double score = (double)per_sm * nw;
-      if (traj) {  // rows of the last tile of a trajectory idle, and halo waypoints cost 2 extra FK per tile
-        const int tiles = (io->horizon + nw - 1) / nw;
-        score *= (double)io->horizon / ((double)tiles * nw + 0.3 * 2.0 * (tiles - 1));
-      }
-      if (score > best_score) {
-        best_score = score;
-        best_nw = nw;
-        best_per_sm = per_sm;
-      }
-    }
-    if (best_nw == 0) return ret(cudaErrorInvalidConfiguration);
-    pl.key = key;
-    pl.nw = best_nw;
-    pl.per_sm = best_per_sm;
-  }
-  const int nw = pl.nw;
-  {
-    const char *qs = getenv("CB200_QUEUE");  // tuning knob: 0 = static striding even when a counter is given
-    a.work_counter = !(qs && atoi(qs) == 0) ? io->work_counter : nullptr;
-    if (traj && (long long)io->batch_size * ((io->horizon + nw - 1) / nw) > 0x3fffffffLL) a.work_counter = nullptr;  // int tickets
-  }
-  const size_t smem = (size_t)h.smem_bytes + halo_bytes + (size_t)nw * warp_floats * sizeof(float);
-  long long grid_ll = (long long)d.sm_count * pl.per_sm;
+  const cudaError_t e =
+      cached_plan(PlanKey{(const void *)kern, d.ordinal, (size_t)h.smem_bytes + halo_bytes, rows_per_warp * a.eval_floats,
+                          traj ? io->horizon : 0, 0, 0},
+                  d, [](const PlanKey &k, size_t limit) { return plan_warps(k, limit, kWarpsPerCta); }, p);
+  if (e != cudaSuccess) return ret(e);
+  if (p.nw == 0) return ret(cudaErrorInvalidConfiguration);
+  const int nw = p.nw;
+  a.work_counter = counter;
+  if (traj && (long long)io->batch_size * ((io->horizon + nw - 1) / nw) > 0x3fffffffLL) a.work_counter = nullptr;  // int tickets
+  long long grid_ll = (long long)d.sm_count * p.per_sm;
   const long long units = (N + rows_per_warp - 1) / rows_per_warp;  // rows, or pairs of rows
   const long long need_ctas = traj ? (long long)io->batch_size * ((io->horizon + nw - 1) / nw) : (units + nw - 1) / nw;
   if (grid_ll > need_ctas) grid_ll = need_ctas;
   const int grid = (int)(grid_ll < 1 ? 1 : grid_ll);
   if (need_ctas <= grid_ll) a.work_counter = nullptr;  // every row / pair / tile has its own warp / CTA: nothing to hand out
-  g_last_variant = traj ? CB200_VARIANT_TRAJ : (variant >= 5 ? CB200_VARIANT_ARM : CB200_VARIANT_STANDARD);
-  CB200_LAUNCH(kern, grid, nw * 32, smem, (cudaStream_t)stream, a);
+  g_last_variant = traj ? CB200_VARIANT_TRAJ : (arm ? CB200_VARIANT_ARM : CB200_VARIANT_STANDARD);
+  CB200_LAUNCH(kern, grid, nw * 32, p.smem, (cudaStream_t)stream, a);
   return finish();
 }
 

@@ -427,7 +427,7 @@ __device__ __forceinline__ float warp_self_collision_tiles(const RobotView &rv, 
       const int sa = rv.cl_start[a], na = rv.cl_start[a + 1] - sa;
       const int sb = rv.cl_start[b], nb = rv.cl_start[b + 1] - sb;
       if (CULL2 && es.ft != nullptr && na <= 32 && nb <= 32 && na * nb > 64) {  // (a block of <= 2 passes is cheaper to scan
-                                                                        // than to cull; the tile schedule has no scratch)
+                                                                        // than to cull; the lists are staged in es.ft)
         // Second-level cull (exact): a pair (i, j) with f > 0 has |p_i - c_b| < r_i + R_b and |p_j - c_a| < r_j + R_a
         // (bounds enclose the padded sphere balls), so only spheres that reach the OTHER link's bound can matter.
         // Most blocks that survive the bound-vs-bound test have none on one side and are dropped here; the rest are

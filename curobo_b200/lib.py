@@ -120,11 +120,7 @@ EXPORTED_SYMBOLS = tuple(_SIGS.keys())
 
 
 def lib_path() -> str:
-    """CB200_LIB_VARIANT=mb3|mb4 selects a register-cap tuning build (same sources, same ABI) if it exists."""
-    d = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib")
-    v = os.environ.get("CB200_LIB_VARIANT", "")
-    p = os.path.join(d, f"libcurobo_b200_{v}.so") if v else ""
-    return p if p and os.path.exists(p) else os.path.join(d, "libcurobo_b200.so")
+    return os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "libcurobo_b200.so")
 
 
 def load() -> C.CDLL:
@@ -133,15 +129,14 @@ def load() -> C.CDLL:
     if _LIB is not None:
         return _LIB
     path = lib_path()
-    if not os.environ.get("CB200_LIB_VARIANT"):
-        # rebuild when a source is newer than the library (cheap mtime check); a box without nvcc -- the GPU box
-        # receives the prebuilt library -- uses what is there and fails loudly below if nothing is
-        from . import build
-        try:
-            build.build_product()
-        except RuntimeError:
-            if not os.path.exists(path):
-                raise
+    # rebuild when a source is newer than the library (cheap mtime check); a box without nvcc -- the GPU box
+    # receives the prebuilt library -- uses what is there and fails loudly below if nothing is
+    from . import build
+    try:
+        build.build_product()
+    except RuntimeError:
+        if not os.path.exists(path):
+            raise
     lib = C.CDLL(path)
     for name, (args, res) in _SIGS.items():
         fn = getattr(lib, name)       # AttributeError if the symbol is missing: fail loudly

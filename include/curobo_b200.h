@@ -44,8 +44,6 @@ const char *cb200_error_string(int err);
 #define CB200_VARIANT_TEAM4 6    /* ... four warps per row */
 #define CB200_VARIANT_TRAJ 7     /* rollout_traj_kernel: trajectory mode (swept collision, state costs) */
 #define CB200_VARIANT_TRAJ_DYN 8 /* rollout_traj_dyn_kernel: trajectory mode + inverse dynamics */
-#define CB200_VARIANT_TILE 9     /* experimental schedules (off by default) */
-#define CB200_VARIANT_LANE 10
 int cb200_last_rollout_variant(void);
 
 /* -------------------------------------------------------------------------------------------
