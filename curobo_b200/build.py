@@ -3,7 +3,7 @@
   curobo_b200/lib/libcurobo_b200.so   -- the product: sm_90a kernels + C ABI (include/curobo_b200.h)
   tests/hostmath/libcb200_hostmath.so -- TEST-ONLY host build of the scalar math (CPU unit tests)
   oracle/_ref/libcurobo_ref.so        -- TEST-ONLY: the reference's own CUDA kernels, compiled from
-                                         /root/reference where they lie (only when that tree exists)
+  oracle/_ref/libcurobo_ref_legacy.so    /root/reference where they lie (only when that tree exists)
 """
 from __future__ import annotations
 
@@ -147,6 +147,22 @@ def build_reference_kernels(force: bool = False, verbose: bool = False):
     return REF_SO
 
 
+def build_reference_legacy_kernels(force: bool = False, verbose: bool = False):
+    """oracle/_ref/libcurobo_ref_legacy.so: the reference's legacy trajectory kernels (POSITION clique, ACCELERATION
+    integration), compiled from the reference tree like build_reference_kernels.  Returns None if the tree is absent."""
+    src = os.path.join(ROOT, "oracle", "ref_legacy_trajectory_launcher.cu")
+    out = os.path.join(os.path.dirname(REF_SO), "libcurobo_ref_legacy.so")
+    kdir = os.path.join(REFERENCE, "curobo", "_src", "curobolib", "kernels")
+    if not os.path.isdir(kdir) or not os.path.exists(src):
+        return out if os.path.exists(out) else None
+    if not force and _newer(out, [src]):
+        return out
+    os.makedirs(os.path.dirname(out), exist_ok=True)
+    _run([_nvcc(), "-std=c++17", "-O3", "-lineinfo", *ARCH, *NUMERIC, "-Xcompiler", "-fPIC", "-shared", "-I", kdir, src, "-o",
+          out, "-lcudart"], verbose)
+    return out
+
+
 def build_reference_callsites(force: bool = False, verbose: bool = False):
     """oracle/_ref/pyref: the reference's Python call sites of the kernel backends (cuda_ops/*.py and their import closure)
     compiled to byte code from the sources where they lie (recipe: oracle/build_pyref.py; test infrastructure, git-ignored,
@@ -164,6 +180,7 @@ def build_reference_callsites(force: bool = False, verbose: bool = False):
 
 def build_all(force: bool = False, verbose: bool = False):
     build_reference_callsites(force, verbose)
+    build_reference_legacy_kernels(force, verbose)
     return build_product(force, verbose), build_hostmath(force, verbose), build_reference_kernels(force, verbose)
 
 

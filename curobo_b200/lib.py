@@ -94,6 +94,9 @@ _SIGS = {
     "cb200_bspline_forward": ([c_p] * 18 + [_I] * 5 + [c_p], _I),
     "cb200_bspline_single_dt": ([c_p] * 20 + [_I] * 5 + [c_p], _I),
     "cb200_bspline_backward": ([c_p] * 8 + [_I] * 5 + [c_p], _I),
+    "cb200_position_clique_forward": ([c_p] * 16 + [_I] * 3 + [c_p], _I),
+    "cb200_position_clique_backward": ([c_p] * 8 + [_I] * 3 + [c_p], _I),
+    "cb200_acceleration_integrate": ([c_p] * 10 + [_I] * 4 + [c_p], _I),
     "cb200_lbfgs_step": ([c_p] * 8 + [C.c_float] + [_I] * 4 + [c_p] * 3 + [_I, c_p, _I, _I, c_p], _I),
     "cb200_line_search": ([c_p] * 5 + [_I, C.c_float, C.c_float] + [c_p] * 13 + [C.c_float, C.c_float] + [_I] * 5 + [c_p], _I),
     "cb200_voxel_mip_block": ([], _I),

@@ -19,6 +19,7 @@ import torch
 from . import lib as _lib
 from .backends.tensor_checks import check_tensors, stream_ptr
 from .backends import tensor_checks as _tc
+from .backends import trajectory as trajectory_cu
 from .robot_model import RobotModel
 from .mesh import c_mesh_set
 from .scene import CuboidData, VoxelData, c_cuboid_set, c_voxel_set
@@ -98,6 +99,7 @@ class RolloutOutput:
     robot_spheres: Optional[torch.Tensor] = None
     pose_goalset_idx: Optional[torch.Tensor] = None
     grad_knots: Optional[torch.Tensor] = None   # [B,n_knots,D] (evaluate_knots only)
+    grad_u: Optional[torch.Tensor] = None       # [B,H-4,D] (evaluate_positions only)
 
 
 def pack_robot_blob(rm: RobotModel) -> np.ndarray:
@@ -371,6 +373,48 @@ class RolloutEngine:
         if self._dyn_params is not None and in_kernel_spline:
             raise ValueError("the dynamics-aware cost needs the expanded spline schedule (in_kernel_spline=False)")
         return self._launch(io, B, H, env_query_idx)
+
+    def evaluate_positions(self, u: torch.Tensor, start_state, start_state_idx: torch.Tensor, goal_state,
+                           goal_state_idx: torch.Tensor, use_implicit_goal_state: torch.Tensor,
+                           env_query_idx: Optional[torch.Tensor] = None) -> RolloutOutput:
+        """Position action space without teleport (the reference's POSITION control space, StateFromPositionClique):
+        waypoints u [B, H-4, D] -> row costs and d cost / d u (`grad_u`).  Three launches on the current stream: the clique
+        stencil (u -> position / velocity / acceleration / jerk [B, H, D] with start-state and implicit-goal padding), the
+        fused rollout in trajectory mode (evaluate_action with those states), the clique adjoint of grad_q / grad_vel /
+        grad_acc / grad_jerk.  start_state / goal_state carry position, velocity, acceleration; goal_state.dt [n_goal] is
+        the trajectory dt; start / goal rows are gathered through start_state_idx / goal_state_idx [B] (same contract as
+        curobo_b200.trajectory.StateFromPositionClique.forward).  The states are kept in `_state` / `_state_dt`; every
+        buffer is allocated once per (B, H), so the call is CUDA-graph capturable."""
+        D = self.robot.num_dof
+        if u.ndim != 3 or u.shape[2] != D:
+            raise ValueError(f"u must be [B, horizon - 4, {D}], got {tuple(u.shape)}")
+        if self.cfg.cspace_type != "state":
+            raise ValueError("evaluate_positions needs the STATE c-space cost (velocity / acceleration / jerk gradients)")
+        if goal_state.dt is None:
+            raise ValueError("dt is None")
+        B, n, _ = u.shape
+        H = n + 4
+        if start_state_idx.shape[0] != B or goal_state_idx.shape[0] != B:
+            raise ValueError("start_state_idx / goal_state_idx need one entry per batch row")
+        dev = self.device
+        if getattr(self, "_state", None) is None or tuple(self._state[0].shape) != (B, H, D):
+            self._state = tuple(torch.zeros((B, H, D), dtype=torch.float32, device=dev) for _ in range(4))
+            self._state_dt = torch.zeros((B,), dtype=torch.float32, device=dev)
+        if (B, H) != (self._B, self._H):
+            self.setup_batch_tensors(B, H)
+        o = self.out
+        if o.grad_u is None or tuple(o.grad_u.shape) != (B, n, D):
+            o.grad_u = torch.zeros((B, n, D), dtype=torch.float32, device=dev)
+        p, v, a, j = self._state
+        trajectory_cu.launch_differentiation_position_forward_kernel(
+            p, v, a, j, self._state_dt, u, start_state.position, start_state.velocity, start_state.acceleration,
+            goal_state.position, goal_state.velocity, goal_state.acceleration, start_state_idx, goal_state_idx, goal_state.dt,
+            use_implicit_goal_state, B, H, D)
+        out = self.evaluate_action(p, vel=v, acc=a, jerk=j, dt=self._state_dt, env_query_idx=env_query_idx)
+        trajectory_cu.launch_differentiation_position_backward_kernel(
+            out.grad_u, out.grad_q, out.grad_vel, out.grad_acc, out.grad_jerk, goal_state.dt, goal_state_idx,
+            use_implicit_goal_state, B, H, D)
+        return out
 
     def _launch(self, io, B: int, H: int, env_query_idx) -> RolloutOutput:
         dev = self.device

@@ -11,9 +11,9 @@ and solvers (GradientOptCore / LBFGSOpt -> IKSolver / TrajOptSolver / MPCSolver)
         c.backward(gradient=ones); g = x.grad
 
 The returned term tensors are outputs of ONE autograd node (`FusedTermsFunction`): forward = one fused launch (two more
-with the B-spline action space), backward hands out the gradient that launch already wrote -- the reference's own contract
-for its cost Functions with use_grad_input=False (cuda_ops/geometry.py:95-104, wp_autograd.py:103-110), so the reference's
-`cat + sum + backward(ones)` yields exactly `grad_q` / `grad_knots`.  Term classification follows the shipped task files
+with the B-spline and position-clique action spaces), backward hands out the gradient that launch already wrote -- the
+reference's own contract for its cost Functions with use_grad_input=False (cuda_ops/geometry.py:95-104,
+wp_autograd.py:103-110), so the reference's `cat + sum + backward(ones)` yields exactly `grad_q` / `grad_knots` / `grad_u`.  Term classification follows the shipped task files
 (content/configs/task/*/lbfgs_*.yml): tool pose and c-space are costs, scene and self collision are constraints.
 
 CUDA only; buffers are allocated once per batch size (update_batch_size), never inside evaluate_action.
@@ -130,7 +130,7 @@ class FusedTermsFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, act_seq: torch.Tensor, rollout: "B200RobotRollout"):
         out = rollout._launch(act_seq.detach())
-        ctx.save_for_backward(out.grad_knots if rollout.is_bspline else out.grad_q)
+        ctx.save_for_backward(out.grad_knots if rollout.is_bspline else out.grad_u if rollout.is_clique else out.grad_q)
         # fresh aliases of the engine's persistent output buffers: autograd attaches this node to the alias objects
         return (out.self_cost.detach().unsqueeze(-1), out.scene_cost.detach(), out.pose_cost.detach(),
                 out.cspace_cost.detach())
@@ -149,23 +149,32 @@ class B200RobotRollout:
     that only integrates positions).
     action space "bspline": act_seq [B, n_knots, D] are B-spline knots; waypoints, their derivatives and d/d knots are
     evaluated by the spline kernels in front of / behind the rollout kernel (RolloutEngine.evaluate_knots;
-    transition/fns_state_transition.py:309-463)."""
+    transition/fns_state_transition.py:309-463).
+    action space "position_clique": act_seq [B, horizon - 4, D] are waypoints; the state [B, horizon, D] and d/d act_seq come
+    from the 5-point stencil with start-state and implicit-goal padding in front of / behind the rollout kernel
+    (RolloutEngine.evaluate_positions; the reference's POSITION control space without teleport,
+    transition/fns_state_transition.py:159-308).  Like "bspline" it needs update_params(start_state=..., goal_state=...)."""
 
     def __init__(self, robot: RobotModel, cfg: RolloutConfig, device="cuda:0", cuboid=None, voxel=None, horizon: int = 1,
                  dt: float = 0.05, action_space: str = "position", n_knots: int = 0, bspline_degree: int = 4,
                  interpolation_steps: int = 4, sum_horizon: bool = True, use_voxel_mip: bool = False, mesh=None):
-        if action_space not in ("position", "bspline"):
-            raise ValueError("action_space must be 'position' or 'bspline'")
+        if action_space not in ("position", "bspline", "position_clique"):
+            raise ValueError("action_space must be 'position', 'bspline' or 'position_clique'")
         self.robot, self.cfg, self.device = robot, cfg, torch.device(device)
         self.engine = RolloutEngine(robot, cfg, device, cuboid, voxel, store_fk_outputs=True, use_voxel_mip=use_voxel_mip,
                                     mesh=mesh)
         self.is_bspline = action_space == "bspline"
+        self.is_clique = action_space == "position_clique"
         self._degree, self._steps = bspline_degree, interpolation_steps
         if self.is_bspline:
             if n_knots < 1:
                 raise ValueError("bspline action space needs n_knots >= 1")
             self._action_horizon = n_knots
             self._horizon = (n_knots + bspline_degree + 1) * interpolation_steps + 1
+        elif self.is_clique:
+            if horizon < 8:
+                raise ValueError(f"position_clique action space needs horizon >= 8, got {horizon}")
+            self._action_horizon, self._horizon = horizon - 4, horizon
         else:
             self._action_horizon = self._horizon = horizon
         self._dt = float(dt)
@@ -229,6 +238,12 @@ class B200RobotRollout:
             return self.engine.evaluate_knots(act_seq, s["start"], s["start_idx"], s["goal"], s["goal_idx"], s["implicit"],
                                               bspline_degree=self._degree, interpolation_steps=self._steps,
                                               env_query_idx=self._env_query_idx)
+        if self.is_clique:
+            s = self._spline_args
+            if s is None:
+                raise ValueError("position_clique action space: call update_params(start_state=..., goal_state=...) first")
+            return self.engine.evaluate_positions(act_seq, s["start"], s["start_idx"], s["goal"], s["goal_idx"], s["implicit"],
+                                                  env_query_idx=self._env_query_idx)
         st = self._state
         if st is not None:
             return self.engine.evaluate_action(act_seq, vel=st.velocity, acc=st.acceleration, jerk=st.jerk, dt=st.dt,
@@ -254,7 +269,7 @@ class B200RobotRollout:
         return cc
 
     def _state_of(self, act_seq: torch.Tensor) -> JointState:
-        if self.is_bspline:
+        if self.is_bspline or self.is_clique:
             p, v, a, j = self.engine._state
             return JointState(p, v, a, j, self.engine._state_dt)
         st = self._state
@@ -285,6 +300,9 @@ class B200RobotRollout:
         """Metrics of a given joint-state trajectory [B, H, D] (position action space semantics)."""
         if self.is_bspline:
             raise ValueError("compute_metrics_from_state: pass knots to compute_metrics_from_action in the bspline action space")
+        if self.is_clique:
+            raise ValueError("compute_metrics_from_state: pass waypoints to compute_metrics_from_action in the position_clique "
+                             "action space")
         prev = self._state
         try:
             if state.velocity is not None and state.acceleration is not None and state.jerk is not None and state.dt is not None:
@@ -334,7 +352,8 @@ class B200RobotRollout:
                       start_state_idx: Optional[torch.Tensor] = None, goal_state_idx: Optional[torch.Tensor] = None,
                       use_implicit_goal_state: Optional[torch.Tensor] = None, **pose_extra) -> bool:
         """Targets of the next solve: tool-pose goals (GoalRegistry rows: goal_* [G, L, n_goalset, 3|4], idxs_goal [B]),
-        the c-space target, the world index per seed, and -- bspline action space -- the boundary states of the spline."""
+        the c-space target, the world index per seed, and -- bspline and position_clique action spaces -- the boundary
+        states of the trajectory."""
         if goal_position is not None:
             self.engine.update_goal(goal_position, goal_quat, idxs_goal, **pose_extra)
         if cspace_target is not None:

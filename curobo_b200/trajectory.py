@@ -5,6 +5,9 @@
                                     same positional arguments)
   get_bspline_interpolation      <- cuda_ops/trajectory.py:21-96 (single-dt resampling of the final trajectory)
   StateFromBSplineKnot           <- curobo/_src/transition/fns_state_transition.py:309-463
+and of its legacy POSITION (clique, non-teleport) and ACCELERATION control spaces:
+  CliqueTensorStepIdxKernel / AccelerationTensorStepIdxKernel <- cuda_ops/trajectory.py:95-296
+  StateFromPositionClique / StateFromAcceleration             <- transition/fns_state_transition.py:90-308
 
 CUDA only, float32 only, like the reference (fns_state_transition.py:323).  No CPU fallback.
 """
@@ -183,4 +186,165 @@ class StateFromBSplineKnot:
                                    out_state_seq.velocity, out_state_seq.acceleration, out_state_seq.jerk,
                                    out_state_seq.dt, goal_state.dt, use_implicit_goal_state, self._u_grad,
                                    self.bspline_degree)
+        return out_state_seq
+
+
+# ------------------------------------------------------------------------------------------------
+# POSITION (clique) and ACCELERATION control spaces
+#   CliqueTensorStepIdxKernel        <- cuda_ops/trajectory.py:95-235
+#   AccelerationTensorStepIdxKernel  <- cuda_ops/trajectory.py:237-296
+#   StateFromPositionClique          <- transition/fns_state_transition.py:159-308
+#   StateFromAcceleration            <- transition/fns_state_transition.py:90-157
+# ------------------------------------------------------------------------------------------------
+class CliqueTensorStepIdxKernel(torch.autograd.Function):
+    """Waypoints u [B, H-4, D] -> (position, velocity, acceleration, jerk) [B, H, D]; backward returns d loss / d u into
+    `out_grad_position`."""
+
+    @staticmethod
+    def forward(ctx, u_act, start_position, start_velocity, start_acceleration, goal_position, goal_velocity,
+                goal_acceleration, start_idx, goal_idx, out_position, out_velocity, out_acceleration, out_jerk, out_dt,
+                traj_dt, use_implicit_goal_state, out_grad_position):
+        horizon = out_position.shape[1]
+        if u_act.shape[-2] != horizon - 4:
+            raise ValueError("Action shape is not compatible with horizon: " + str(u_act.shape))
+        trajectory_cu.launch_differentiation_position_forward_kernel(
+            out_position, out_velocity, out_acceleration, out_jerk, out_dt, u_act, start_position, start_velocity,
+            start_acceleration, goal_position, goal_velocity, goal_acceleration, start_idx, goal_idx, traj_dt,
+            use_implicit_goal_state, out_position.shape[0], out_position.shape[1], out_position.shape[-1])
+        if ctx.needs_input_grad[0]:
+            ctx.save_for_backward(traj_dt, out_grad_position, goal_idx, use_implicit_goal_state)
+        return out_position, out_velocity, out_acceleration, out_jerk
+
+    @staticmethod
+    def backward(ctx, grad_out_p, grad_out_v, grad_out_a, grad_out_j):
+        u_grad = None
+        if ctx.needs_input_grad[0]:
+            traj_dt, out_grad_position, goal_idx, use_implicit_goal_state = ctx.saved_tensors
+            for name, g in (("grad_out_p", grad_out_p), ("grad_out_v", grad_out_v), ("grad_out_a", grad_out_a),
+                            ("grad_out_j", grad_out_j)):
+                if g is None:
+                    raise ValueError(f"{name} is None")
+            trajectory_cu.launch_differentiation_position_backward_kernel(
+                out_grad_position, grad_out_p.contiguous(), grad_out_v.contiguous(), grad_out_a.contiguous(),
+                grad_out_j.contiguous(), traj_dt, goal_idx, use_implicit_goal_state, grad_out_p.shape[0],
+                grad_out_p.shape[1], grad_out_p.shape[2])
+            u_grad = out_grad_position
+        return (u_grad,) + (None,) * 16
+
+
+class AccelerationTensorStepIdxKernel(torch.autograd.Function):
+    """Accelerations u [B, H, D] -> (position, velocity, acceleration, jerk) [B, H, D]; no backward, like the reference."""
+
+    @staticmethod
+    def forward(ctx, u_act, start_position, start_velocity, start_acceleration, start_idx, out_position, out_velocity,
+                out_acceleration, out_jerk, traj_dt, out_grad_position):
+        trajectory_cu.launch_integration_acceleration_kernel(
+            out_position, out_velocity, out_acceleration, out_jerk, u_act, start_position, start_velocity,
+            start_acceleration, start_idx, traj_dt, out_position.shape[0], out_position.shape[1], out_position.shape[-1],
+            True)
+        ctx.save_for_backward(traj_dt, out_grad_position)
+        return out_position, out_velocity, out_acceleration, out_jerk
+
+    @staticmethod
+    def backward(ctx, grad_out_p, grad_out_v, grad_out_a, grad_out_j):
+        if ctx.needs_input_grad[0]:
+            raise NotImplementedError()
+        return (None,) * 11
+
+
+def _no_filters(filter_velocity: bool, filter_acceleration: bool, filter_jerk: bool) -> None:
+    if filter_velocity or filter_acceleration or filter_jerk:
+        raise ValueError("the moving-average filters of the clique state (filter_velocity / filter_acceleration / "
+                         "filter_jerk) are not supported")
+
+
+class StateFromPositionClique:
+    """Action (waypoints [B, H-4, D]) -> state sequence [B, H, D] by the 5-point stencil (position control space without
+    teleport).  `dt_h` is kept for update_dt like the reference's; the stencil reads dt from goal_state.dt."""
+
+    def __init__(self, device: torch.device, dt_h: torch.Tensor, dof: int, filter_velocity: bool = False,
+                 filter_acceleration: bool = False, filter_jerk: bool = False, batch_size: int = 1,
+                 horizon: int = 1) -> None:
+        _no_filters(filter_velocity, filter_acceleration, filter_jerk)
+        self.device = torch.device(device)
+        self.dof = dof
+        self._dt_h = dt_h
+        self._inv_dt_h = 1.0 / dt_h
+        self._u_grad = None
+        self.batch_size = self.horizon = -1
+        self.update_batch_size(batch_size, horizon)
+
+    def update_dt(self, dt: float) -> None:
+        self._dt_h[:] = dt
+        self._inv_dt_h[:] = 1.0 / dt
+
+    def update_batch_size(self, batch_size: Optional[int] = None, horizon: Optional[int] = None,
+                          force_update: bool = False) -> None:
+        if batch_size != self.batch_size or horizon != self.horizon or self._u_grad is None:
+            self.action_horizon = horizon - 4
+            self._u_grad = torch.zeros((batch_size, self.action_horizon, self.dof), device=self.device, dtype=torch.float32)
+        if force_update:
+            self._u_grad = self._u_grad.detach()
+        self.batch_size, self.horizon = batch_size, horizon
+
+    def forward(self, start_state: JointState, u_act: torch.Tensor, out_state_seq: JointState,
+                start_state_idx: Optional[torch.Tensor] = None, goal_state: Optional[JointState] = None,
+                goal_state_idx: Optional[torch.Tensor] = None, use_implicit_goal_state: Optional[torch.Tensor] = None,
+                **kwargs) -> JointState:
+        # argument checks of fns_state_transition.py:260-277
+        if start_state_idx is None:
+            raise ValueError("Start state index is required for Clique kernel")
+        if goal_state is None:
+            goal_state = start_state
+        if goal_state_idx is None:
+            goal_state_idx = start_state_idx
+        if goal_state.dt.shape != goal_state.position.shape[0:2]:
+            raise ValueError(f"Shape mismatch: goal_state.dt.shape[0] != goal_state.position.shape[0:2]: "
+                             f"{goal_state.dt.shape} != {goal_state.position.shape[0:2]}")
+        if use_implicit_goal_state.shape != goal_state.position.shape[0:2]:
+            raise ValueError(f"Shape mismatch: use_implicit_goal_state.shape[0] != goal_state.position.shape[0]: "
+                             f"{use_implicit_goal_state.shape[0]} != "
+                             f"{goal_state.position.view(-1, goal_state.position.shape[-1]).shape[0]}")
+        (out_state_seq.position, out_state_seq.velocity, out_state_seq.acceleration, out_state_seq.jerk) = \
+            CliqueTensorStepIdxKernel.apply(u_act, start_state.position, start_state.velocity, start_state.acceleration,
+                                            goal_state.position, goal_state.velocity, goal_state.acceleration,
+                                            start_state_idx, goal_state_idx, out_state_seq.position,
+                                            out_state_seq.velocity, out_state_seq.acceleration, out_state_seq.jerk,
+                                            out_state_seq.dt, goal_state.dt, use_implicit_goal_state, self._u_grad)
+        return out_state_seq
+
+
+class StateFromAcceleration:
+    """Action (accelerations [B, H, D]) -> state sequence [B, H, D] by semi-implicit Euler with dt[h] = dt_h[h]."""
+
+    def __init__(self, device: torch.device, dt_h: torch.Tensor, dof: int, batch_size: int = 1, horizon: int = 1) -> None:
+        self.device = torch.device(device)
+        self.dof = dof
+        self._dt_h = dt_h
+        self._inv_dt_h = None
+        self.batch_size = self.horizon = -1
+        self.action_horizon = horizon
+        self._u_grad = torch.zeros((batch_size, horizon, dof), device=self.device, dtype=torch.float32)
+        self.batch_size, self.horizon = batch_size, horizon
+
+    def update_dt(self, dt: float) -> None:
+        self._dt_h[:] = dt
+
+    def update_batch_size(self, batch_size: Optional[int] = None, horizon: Optional[int] = None,
+                          force_update: bool = False) -> None:
+        if batch_size != self.batch_size or horizon != self.horizon:
+            self._u_grad = torch.zeros((batch_size, horizon, self.dof), device=self.device, dtype=torch.float32)
+        if force_update:
+            self._u_grad = self._u_grad.detach()
+        self.batch_size, self.horizon = batch_size, horizon
+
+    def forward(self, start_state: JointState, u_act: torch.Tensor, out_state_seq: JointState,
+                start_state_idx: Optional[torch.Tensor] = None, **kwargs) -> JointState:
+        if start_state_idx is None:
+            raise ValueError("Start state index is required for Acceleration kernel")
+        (out_state_seq.position, out_state_seq.velocity, out_state_seq.acceleration, out_state_seq.jerk) = \
+            AccelerationTensorStepIdxKernel.apply(u_act, start_state.position, start_state.velocity,
+                                                  start_state.acceleration, start_state_idx, out_state_seq.position,
+                                                  out_state_seq.velocity, out_state_seq.acceleration, out_state_seq.jerk,
+                                                  self._dt_h, self._u_grad)
         return out_state_seq

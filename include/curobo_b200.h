@@ -399,6 +399,44 @@ int cb200_bspline_backward(
     int dof, int n_knots, int bspline_degree, cb200_stream_t stream);
 
 /* -------------------------------------------------------------------------------------------
+ * Position (clique) and acceleration control spaces: the reference's legacy state transitions
+ * (kernels/trajectory/legacy/).  Argument order and meaning are the reference launchers':
+ *   cb200_position_clique_forward  <- launch_differentiation_position_forward_kernel
+ *       curobo/_src/curobolib/backends/cuda_core_backend/trajectory.py:309-393
+ *       (pybind twin: backends/pybind/trajectory_kernel_launch.cu:26-107)
+ *   cb200_position_clique_backward <- launch_differentiation_position_backward_kernel  trajectory.py:396-465
+ *   cb200_acceleration_integrate   <- launch_integration_acceleration_kernel           trajectory.py:468-560
+ * Clique: u_position [B, H-4, D] -> position / velocity / acceleration / jerk [B, H, D] by the 5-point stencil,
+ * padded with the start state before the first action and with the last action (or, where
+ * use_implicit_goal_state[goal_idx[b]], the goal position) after it; out_dt [B] = traj_dt[goal_idx[b]].
+ * start_* / goal_* are gathered at flat offsets start_idx[b] * D / goal_idx[b] * D.  The adjoint maps the four
+ * [B, H, D] gradients to out_grad_position [B, H-4, D]; dt and the goal mode come through dt_idx[b].
+ * Both return cudaErrorInvalidValue for horizon < 8 (the reference's first rows read actions 0..3 whatever the
+ * horizon).
+ * Acceleration: u_acc [B, H, D] -> the four state tensors [B, H, D] by semi-implicit Euler with dt[h] = traj_dt[h]
+ * ([H], indexed by waypoint); the start state comes through start_idx.  use_rk2 selects a kernel with identical
+ * arithmetic in the reference and is accepted for either value.  No horizon limit.
+ * batch_size == 0 returns cudaSuccess without launching.
+ * ------------------------------------------------------------------------------------------- */
+int cb200_position_clique_forward(
+    float *out_position, float *out_velocity, float *out_acceleration, float *out_jerk, float *out_dt,
+    const float *u_position, const float *start_position, const float *start_velocity,
+    const float *start_acceleration, const float *goal_position, const float *goal_velocity,
+    const float *goal_acceleration, const int32_t *start_idx, const int32_t *goal_idx, const float *traj_dt,
+    const uint8_t *use_implicit_goal_state, int batch_size, int horizon, int dof, cb200_stream_t stream);
+
+int cb200_position_clique_backward(
+    float *out_grad_position, const float *grad_position, const float *grad_velocity,
+    const float *grad_acceleration, const float *grad_jerk, const float *traj_dt, const int32_t *dt_idx,
+    const uint8_t *use_implicit_goal_state, int batch_size, int horizon, int dof, cb200_stream_t stream);
+
+int cb200_acceleration_integrate(
+    float *out_position, float *out_velocity, float *out_acceleration, float *out_jerk, const float *u_acc,
+    const float *start_position, const float *start_velocity, const float *start_acceleration,
+    const int32_t *start_idx, const float *traj_dt, int batch_size, int horizon, int dof, int use_rk2,
+    cb200_stream_t stream);
+
+/* -------------------------------------------------------------------------------------------
  * (8f-2) Optimizer-side kernels of the solve loop: the L-BFGS step and the parallel Wolfe line search
  * that sit either side of the rollout in every optimizer iteration.
  *   cb200_lbfgs_step   <- launch_lbfgs_step
