@@ -207,16 +207,18 @@ __device__ __forceinline__ float cspace_dof(const FusedArgs &a, const RobotView 
 }
 
 // ------------------------------------------------------------------------------------------------
-// Row phases shared by the two fused kernels.
+// Row phases shared by the fused kernels.
 //   phase A: q load + c-space cost, FK, spheres (+ padded copy), tool poses + tool-pose cost
 //   phase B: self collision, scene collision (discrete | swept + speed metric), J^T backward, row cost
+// The helpers are inlined: out-of-line phases needed fewer registers and ran slower (DESIGN.md section 4).
 // ------------------------------------------------------------------------------------------------
+
+// c-space phase of row (b, h): loads the row state into es.qv, the position gradient into es.gqv; returns the lane's cost sum
 template <bool SPLINE, int W = 32>
-__device__ __forceinline__ void row_phase_a(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e,
-                                            int b, int h, float &cs_cost, float &pose_c) {
-  const cb200_rollout_cfg &cfg = a.cfg;
-  const int D = rv.D, S = rv.S, L = rv.L;
-  cs_cost = 0.0f;
+__device__ __forceinline__ float row_cspace(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e, int b,
+                                            int h) {
+  const int D = rv.D;
+  float cs_cost = 0.0f;
   #pragma unroll 1
   for (int d = lane; d < D; d += W) {
     const bspline::State4 st = load_row_state<SPLINE>(a, e, b, h, d, D);
@@ -227,11 +229,17 @@ __device__ __forceinline__ void row_phase_a(const FusedArgs &a, const RobotView 
     cs_cost += c;
     if (a.cspace_cost) a.cspace_cost[(size_t)e * D + d] = c;
   }
-  row_sync<W>();
-  warp_fk<W>(rv, es, lane);
-  warp_spheres<W>(rv, es, lane, a.robot_spheres ? reinterpret_cast<float4 *>(a.robot_spheres) + (size_t)e * S : nullptr,
-                  row_sphere_cfg(a, b, S));
-  pose_c = 0.0f;
+  return cs_cost;
+}
+
+// tool poses of row (b, h) (link_pos / link_quat) and the tool-pose cost: its gradient goes to es.pose_g; returns the lane's
+// cost sum
+template <int W = 32>
+__device__ __forceinline__ float row_tool_poses(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e, int b,
+                                                int h) {
+  const cb200_rollout_cfg &cfg = a.cfg;
+  const int L = rv.L;
+  float pose_c = 0.0f;
   const bool do_pose = (a.goal_position != nullptr);
   #pragma unroll 1
   for (int t = lane; t < L; t += W) {
@@ -272,6 +280,19 @@ __device__ __forceinline__ void row_phase_a(const FusedArgs &a, const RobotView 
       if (a.pose_goalset_idx) a.pose_goalset_idx[(size_t)e * L + t] = po.goal_idx;
     }
   }
+  return pose_c;
+}
+
+template <bool SPLINE, int W = 32>
+__device__ __forceinline__ void row_phase_a(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e,
+                                            int b, int h, float &cs_cost, float &pose_c) {
+  const int S = rv.S;
+  cs_cost = row_cspace<SPLINE, W>(a, rv, es, lane, e, b, h);
+  row_sync<W>();
+  warp_fk<W>(rv, es, lane);
+  warp_spheres<W>(rv, es, lane, a.robot_spheres ? reinterpret_cast<float4 *>(a.robot_spheres) + (size_t)e * S : nullptr,
+                  row_sphere_cfg(a, b, S));
+  pose_c = row_tool_poses<W>(a, rv, es, lane, e, b, h);
   row_sync<W>();
 }
 
@@ -281,6 +302,54 @@ struct RowB1 {
   float self_c, fmax, scene_c;
   int bi, bj, nnz;
 };
+
+// Cuboids of the row's environment (ce, ncub clamped to the set's capacity) and whether the broad phase culls them.
+struct CuboidCull {
+  int ce, ncub;
+  bool cull;
+};
+// Whether the row has cuboid terms.  The mesh build, SCENE = 7, runs with or without cuboids and ESDF grids: it checks at run
+// time which sets are present.
+template <int SCENE>
+__device__ __forceinline__ bool has_cuboids(const FusedArgs &a, bool do_scene) {
+  return (SCENE & 1) && do_scene && (!(SCENE & 4) || a.cuboids.inv_pose != nullptr);
+}
+// Fills cc when has_cuboids; returns cc.cull.  The callers keep this split from has_cuboids, with the mask fill nested inside
+// it: folding the two into one helper changed the register allocation of kernels that have no cuboid terms at all.
+__device__ __forceinline__ bool cuboid_cull_state(const FusedArgs &a, const RobotView &rv, int env, bool discrete, CuboidCull &cc) {
+  cc.ce = env < a.cuboids.num_envs ? env : 0;
+  cc.ncub = a.cuboids.count[cc.ce];
+  if (cc.ncub > a.cuboids.max_n) cc.ncub = a.cuboids.max_n;
+  cc.cull = discrete && rv.n_lp > 0 && cc.ncub <= 32;  // (one mask bit per cuboid)
+  return cc.cull;
+}
+
+// Cuboid broad phase (discrete mode): es.cmask[ca] = the cuboids collision link ca may touch, for ca = first, first + stride, ...
+// A box SDF is 1-Lipschitz, so sdf(link bound centre) >= R_link + eta means no sphere of the link has pen = r + eta - sdf > 0
+// against that cuboid: skipping it is exact.  The caller synchronises its lanes before the masks are read.
+__device__ __forceinline__ void cuboid_cull_masks(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int ce, int ncub,
+                                                  int first, int stride) {
+#pragma unroll 1
+  for (int ca = first; ca < rv.n_cl; ca += stride) {
+    const float4 cb = rv.cl_bound_scene[ca];
+    uint32_t mask = 0u;
+    if (cb.w >= 0.0f) {
+      const float *Tk = es.cumul + 12 * rv.cl_link[ca];
+      const V3 cw = mk3(Tk[0] * cb.x + Tk[1] * cb.y + Tk[2] * cb.z + Tk[3], Tk[4] * cb.x + Tk[5] * cb.y + Tk[6] * cb.z + Tk[7],
+                        Tk[8] * cb.x + Tk[9] * cb.y + Tk[10] * cb.z + Tk[11]);
+#pragma unroll 1
+      for (int i = 0; i < ncub; ++i) {
+        const int kk = ce * a.cuboids.max_n + i;
+        if (a.cuboids.enable[kk] != 1) continue;
+        const ObsFrame f = load_obs_frame(a.cuboids.inv_pose + 8 * kk);
+        const SdfGrad sg = cuboid_sdf_grad(to_obstacle(f, cw), ldgf(a.cuboids.dims + 4 * kk), ldgf(a.cuboids.dims + 4 * kk + 1),
+                                           ldgf(a.cuboids.dims + 4 * kk + 2));
+        if (sg.sdf < cb.w + a.cfg.scene_activation) mask |= (1u << i);
+      }
+    }
+    es.cmask[ca] = mask;
+  }
+}
 
 // Mesh terms of one sphere (the SCENE & 4 builds): weighted world-frame gradient in xyz, weighted cost in w.  The caller adds them
 // to the cuboid + ESDF sum: the order of the per-operator composition, where one launch writes the cuboid + ESDF terms and the
@@ -294,6 +363,50 @@ __device__ __forceinline__ float4 mesh_terms(const MeshSet *ms, float eta, float
   const float cost = sweep ? sphere_scene_swept<4>(c, r, eta, w, has_prev, prev, has_next, next, no_cuboids, no_voxels, env, g, ms)
                            : sphere_scene_discrete<4>(c, r, eta, w, no_cuboids, no_voxels, env, g, ms);
   return make_float4(g.x, g.y, g.z, cost);
+}
+
+// Discrete scene terms of sphere s: the cuboids the broad phase kept, the ESDF grids, the meshes.  Returns the weighted cost and
+// adds the weighted world-frame gradient to g.
+template <int SCENE>
+__device__ __forceinline__ float sphere_discrete_terms(const FusedArgs &a, const RobotView &rv, const EvalSmem &es,
+                                                       const CuboidCull &cc, int env, int s, V3 &g) {
+  const cb200_rollout_cfg &cfg = a.cfg;
+  const float4 sp = es.sph[s];
+  const V3 cen = mk3(sp.x, sp.y, sp.z);
+  float c = 0.0f;
+  if (sp.w >= 0.0f) {
+    if (SCENE & 1) {
+      uint32_t m = cc.cull ? es.cmask[rv.sph_cl[s]] : 0xffffffffu;
+      const float radj = sp.w + cfg.scene_activation;
+#pragma unroll 1
+      for (int i = 0; i < cc.ncub && m != 0u; ++i) {
+        if (cc.cull && !((m >> i) & 1u)) continue;
+        if (cc.cull) m &= ~(1u << i);
+        const int kk = cc.ce * a.cuboids.max_n + i;
+        if (a.cuboids.enable[kk] != 1) continue;
+        const ObsFrame f = load_obs_frame(a.cuboids.inv_pose + 8 * kk);
+        const SdfGrad sg = cuboid_sdf_grad(to_obstacle(f, cen), ldgf(a.cuboids.dims + 4 * kk), ldgf(a.cuboids.dims + 4 * kk + 1),
+                                           ldgf(a.cuboids.dims + 4 * kk + 2));
+        const float pen = radj - sg.sdf;
+        if (pen > 0.0f) {
+          float ac, as;
+          collision_activation(pen, cfg.scene_activation, ac, as);
+          c += cfg.scene_weight * ac;
+          g = g + (cfg.scene_weight * as) * from_obstacle(f, sg.n);
+        }
+      }
+    }
+    if (SCENE & 2) {
+      const CuboidSet none{};
+      c += sphere_scene_discrete<2>(cen, sp.w, cfg.scene_activation, cfg.scene_weight, none, a.voxels, env, g);
+    }
+    if (SCENE & 4) {
+      const float4 m = mesh_terms(&a.meshes, cfg.scene_activation, cfg.scene_weight, cen, sp.w, env, false, false, cen, false, cen);
+      c += m.w;
+      g = g + mk3(m.x, m.y, m.z);
+    }
+  }
+  return c;
 }
 
 template <bool SWEEP, int SCENE, bool CULL2 = true, int W = 32>
@@ -316,37 +429,10 @@ __device__ __forceinline__ RowB1 row_phase_b1(const FusedArgs &a, const RobotVie
   const float sdt = (SWEEP && cfg.use_speed_metric && (a.dt != nullptr || a.spl.knots != nullptr))
                         ? (a.spl.knots != nullptr ? __ldg(a.spl.traj_dt + __ldg(a.spl.goal_idx)) : __ldg(a.dt))
                         : 0.0f;
-  // cuboid broad phase (discrete mode): a box SDF is 1-Lipschitz, so sdf(link bound centre) >= R_link + eta
-  // means no sphere of the link has pen = r + eta - sdf > 0 against that cuboid -> skipping it is exact.
-  // (The mesh build, SCENE = 7, runs with or without cuboids and ESDF grids: it checks at run time which sets are present.)
-  int ce = 0, ncub = 0;
-  bool cull = false;
-  if ((SCENE & 1) && do_scene && (!(SCENE & 4) || a.cuboids.inv_pose != nullptr)) {
-    ce = env < a.cuboids.num_envs ? env : 0;
-    ncub = a.cuboids.count[ce];
-    if (ncub > a.cuboids.max_n) ncub = a.cuboids.max_n;
-    cull = !SWEEP && rv.n_lp > 0 && ncub <= 32;
-    if (cull) {
-#pragma unroll 1
-      for (int ca = lane; ca < rv.n_cl; ca += W) {
-        const float4 cb = rv.cl_bound_scene[ca];
-        uint32_t mask = 0u;
-        if (cb.w >= 0.0f) {
-          const float *Tk = es.cumul + 12 * rv.cl_link[ca];
-          const V3 cw = mk3(Tk[0] * cb.x + Tk[1] * cb.y + Tk[2] * cb.z + Tk[3], Tk[4] * cb.x + Tk[5] * cb.y + Tk[6] * cb.z + Tk[7],
-                            Tk[8] * cb.x + Tk[9] * cb.y + Tk[10] * cb.z + Tk[11]);
-#pragma unroll 1
-          for (int i = 0; i < ncub; ++i) {
-            const int kk = ce * a.cuboids.max_n + i;
-            if (a.cuboids.enable[kk] != 1) continue;
-            const ObsFrame f = load_obs_frame(a.cuboids.inv_pose + 8 * kk);
-            const SdfGrad sg = cuboid_sdf_grad(to_obstacle(f, cw), ldgf(a.cuboids.dims + 4 * kk), ldgf(a.cuboids.dims + 4 * kk + 1),
-                                               ldgf(a.cuboids.dims + 4 * kk + 2));
-            if (sg.sdf < cb.w + cfg.scene_activation) mask |= (1u << i);
-          }
-        }
-        es.cmask[ca] = mask;
-      }
+  CuboidCull cc{0, 0, false};
+  if (has_cuboids<SCENE>(a, do_scene)) {
+    if (cuboid_cull_state(a, rv, env, !SWEEP, cc)) {
+      cuboid_cull_masks(a, rv, es, cc.ce, cc.ncub, lane, W);
       row_sync<W>();
     }
   }
@@ -355,42 +441,11 @@ __device__ __forceinline__ RowB1 row_phase_b1(const FusedArgs &a, const RobotVie
     V3 g = mk3(0, 0, 0);
     float c = 0.0f;
     if (do_scene) {
-      const float4 sp = es.sph[s];
-      const V3 cen = mk3(sp.x, sp.y, sp.z);
       if (!SWEEP) {
-        if (sp.w >= 0.0f) {
-          if (SCENE & 1) {
-            uint32_t m = cull ? es.cmask[rv.sph_cl[s]] : 0xffffffffu;
-            const float radj = sp.w + cfg.scene_activation;
-#pragma unroll 1
-            for (int i = 0; i < ncub && m != 0u; ++i) {
-              if (cull && !((m >> i) & 1u)) continue;
-              if (cull) m &= ~(1u << i);
-              const int kk = ce * a.cuboids.max_n + i;
-              if (a.cuboids.enable[kk] != 1) continue;
-              const ObsFrame f = load_obs_frame(a.cuboids.inv_pose + 8 * kk);
-              const SdfGrad sg = cuboid_sdf_grad(to_obstacle(f, cen), ldgf(a.cuboids.dims + 4 * kk), ldgf(a.cuboids.dims + 4 * kk + 1),
-                                                 ldgf(a.cuboids.dims + 4 * kk + 2));
-              const float pen = radj - sg.sdf;
-              if (pen > 0.0f) {
-                float ac, as;
-                collision_activation(pen, cfg.scene_activation, ac, as);
-                c += cfg.scene_weight * ac;
-                g = g + (cfg.scene_weight * as) * from_obstacle(f, sg.n);
-              }
-            }
-          }
-          if (SCENE & 2) {
-            const CuboidSet none{};
-            c += sphere_scene_discrete<2>(cen, sp.w, cfg.scene_activation, cfg.scene_weight, none, a.voxels, env, g);
-          }
-          if (SCENE & 4) {
-            const float4 m = mesh_terms(&a.meshes, cfg.scene_activation, cfg.scene_weight, cen, sp.w, env, false, false, cen, false, cen);
-            c += m.w;
-            g = g + mk3(m.x, m.y, m.z);
-          }
-        }
+        c = sphere_discrete_terms<SCENE>(a, rv, es, cc, env, s, g);
       } else {
+        const float4 sp = es.sph[s];
+        const V3 cen = mk3(sp.x, sp.y, sp.z);
         V3 pv = cen, nx = cen;
         if (prev_sph != nullptr) {
           const float4 t = prev_sph[s];
@@ -448,6 +503,24 @@ __device__ __forceinline__ void row_phase_b2(const FusedArgs &a, const RobotView
   row_sync<W>();
 }
 
+// Ticket counter [2] of the persistent kernels (FusedArgs::work_counter): [0] hands out work units after each worker's first,
+// [1] counts the workers (warps, teams or CTAs) that have left.  It is zero between launches.
+// Next work unit of a warp that just finished unit u: a ticket when the caller passed a counter, else static striding.
+__device__ __forceinline__ int next_warp_unit(int32_t *counter, int u, int stride, bool leader) {
+  if (counter == nullptr) return u + stride;
+  int nxt = 0;
+  if (leader) nxt = stride + atomicAdd(counter, 1);
+  return __shfl_sync(kFull, nxt, 0);
+}
+// Called once per worker on its way out: the last of `workers` to leave re-arms the counter for the next launch on the stream.
+__device__ __forceinline__ void rearm_ticket_counter(int32_t *counter, int workers) {
+  __threadfence();
+  if (atomicAdd(counter + 1, 1) == workers - 1) {
+    counter[0] = 0;
+    counter[1] = 0;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // THE fused kernel, discrete scene collision: rows are independent, one persistent warp per row, phases
 // inlined (measured best: out-of-line phases needed fewer registers and ran slower).
@@ -487,21 +560,9 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB) rollout_fused_kernel(
       const RowB1 r = row_phase_b1<false, SCENE, MINB != 3, W>(a, rv, es, lane, e, b, nullptr, nullptr);
       row_phase_b2<MINB == 3, W>(a, rv, es, smem, lane, e, r, cs_cost, pose_c);
     }
-    if (a.work_counter != nullptr) {
-      int nxt = 0;
-      if (leader) nxt = stride + atomicAdd(a.work_counter, 1);
-      u = __shfl_sync(kFull, nxt, 0);
-    } else {
-      u += stride;
-    }
+    u = next_warp_unit(a.work_counter, u, stride, leader);
   }
-  if (a.work_counter != nullptr && leader) {  // the last warp to leave re-arms the counter for the next launch
-    __threadfence();
-    if (atomicAdd(a.work_counter + 1, 1) == stride - 1) {
-      a.work_counter[0] = 0;
-      a.work_counter[1] = 0;
-    }
-  }
+  if (a.work_counter != nullptr && leader) rearm_ticket_counter(a.work_counter, stride);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -533,34 +594,10 @@ __device__ __forceinline__ RowB1 row_phase_b1_list(const FusedArgs &a, const Rob
   __syncwarp();
   const bool do_scene = SCENE != 0 && cfg.scene_weight > 0.0f;
   const int env = (a.env_query_idx != nullptr) ? __ldg(a.env_query_idx + b) : 0;
-  int ce = 0, ncub = 0;
-  bool cull = false;
-  if ((SCENE & 1) && do_scene && (!(SCENE & 4) || a.cuboids.inv_pose != nullptr)) {  // cuboid broad phase, as in row_phase_b1
-    ce = env < a.cuboids.num_envs ? env : 0;
-    ncub = a.cuboids.count[ce];
-    if (ncub > a.cuboids.max_n) ncub = a.cuboids.max_n;
-    cull = rv.n_lp > 0 && ncub <= 32;
-    if (cull) {
-#pragma unroll 1
-      for (int ca = lane; ca < rv.n_cl; ca += 32) {
-        const float4 cb = rv.cl_bound_scene[ca];
-        uint32_t mask = 0u;
-        if (cb.w >= 0.0f) {
-          const float *Tk = es.cumul + 12 * rv.cl_link[ca];
-          const V3 cw = mk3(Tk[0] * cb.x + Tk[1] * cb.y + Tk[2] * cb.z + Tk[3], Tk[4] * cb.x + Tk[5] * cb.y + Tk[6] * cb.z + Tk[7],
-                            Tk[8] * cb.x + Tk[9] * cb.y + Tk[10] * cb.z + Tk[11]);
-#pragma unroll 1
-          for (int i = 0; i < ncub; ++i) {
-            const int kk = ce * a.cuboids.max_n + i;
-            if (a.cuboids.enable[kk] != 1) continue;
-            const ObsFrame f = load_obs_frame(a.cuboids.inv_pose + 8 * kk);
-            const SdfGrad sg = cuboid_sdf_grad(to_obstacle(f, cw), ldgf(a.cuboids.dims + 4 * kk), ldgf(a.cuboids.dims + 4 * kk + 1),
-                                               ldgf(a.cuboids.dims + 4 * kk + 2));
-            if (sg.sdf < cb.w + cfg.scene_activation) mask |= (1u << i);
-          }
-        }
-        es.cmask[ca] = mask;
-      }
+  CuboidCull cc{0, 0, false};
+  if (has_cuboids<SCENE>(a, do_scene)) {
+    if (cuboid_cull_state(a, rv, env, true, cc)) {
+      cuboid_cull_masks(a, rv, es, cc.ce, cc.ncub, lane, 32);
       __syncwarp();
     }
   }
@@ -571,42 +608,7 @@ __device__ __forceinline__ RowB1 row_phase_b1_list(const FusedArgs &a, const Rob
     const int s = base + lane;
     V3 g = mk3(0, 0, 0);
     float c = 0.0f;
-    if (s < S && do_scene) {
-      const float4 sp = es.sph[s];
-      const V3 cen = mk3(sp.x, sp.y, sp.z);
-      if (sp.w >= 0.0f) {
-        if (SCENE & 1) {
-          uint32_t m = cull ? es.cmask[rv.sph_cl[s]] : 0xffffffffu;
-          const float radj = sp.w + cfg.scene_activation;
-#pragma unroll 1
-          for (int i = 0; i < ncub && m != 0u; ++i) {
-            if (cull && !((m >> i) & 1u)) continue;
-            if (cull) m &= ~(1u << i);
-            const int kk = ce * a.cuboids.max_n + i;
-            if (a.cuboids.enable[kk] != 1) continue;
-            const ObsFrame f = load_obs_frame(a.cuboids.inv_pose + 8 * kk);
-            const SdfGrad sg = cuboid_sdf_grad(to_obstacle(f, cen), ldgf(a.cuboids.dims + 4 * kk), ldgf(a.cuboids.dims + 4 * kk + 1),
-                                               ldgf(a.cuboids.dims + 4 * kk + 2));
-            const float pen = radj - sg.sdf;
-            if (pen > 0.0f) {
-              float ac, as;
-              collision_activation(pen, cfg.scene_activation, ac, as);
-              c += cfg.scene_weight * ac;
-              g = g + (cfg.scene_weight * as) * from_obstacle(f, sg.n);
-            }
-          }
-        }
-        if (SCENE & 2) {
-          const CuboidSet none{};
-          c += sphere_scene_discrete<2>(cen, sp.w, cfg.scene_activation, cfg.scene_weight, none, a.voxels, env, g);
-        }
-        if (SCENE & 4) {
-          const float4 m = mesh_terms(&a.meshes, cfg.scene_activation, cfg.scene_weight, cen, sp.w, env, false, false, cen, false, cen);
-          c += m.w;
-          g = g + mk3(m.x, m.y, m.z);
-        }
-      }
-    }
+    if (s < S && do_scene) c = sphere_discrete_terms<SCENE>(a, rv, es, cc, env, s, g);
     const bool nz = (g.x != 0.0f) || (g.y != 0.0f) || (g.z != 0.0f);
     const unsigned m = __ballot_sync(kFull, nz);
     if (m) {
@@ -631,18 +633,24 @@ __device__ __forceinline__ RowB1 row_phase_b1_list(const FusedArgs &a, const Rob
   return r;
 }
 
+// the worst self-collision pair's gradient: two more entries of a gradient list (lane 0 writes them, the caller synchronises)
+__device__ __forceinline__ void append_self_pair(const FusedArgs &a, const EvalSmem &es, int lane, int bi, int bj, float4 *list,
+                                                 int &n_list) {
+  if (lane == 0) {
+    const float4 pi = es.sph[bi], pj = es.sph[bj];
+    const float w = a.cfg.self_weight;
+    const float gx = w * (pj.x - pi.x), gy = w * (pj.y - pi.y), gz = w * (pj.z - pi.z);
+    list[n_list] = make_float4(gx, gy, gz, __int_as_float(bi));
+    list[n_list + 1] = make_float4(-gx, -gy, -gz, __int_as_float(bj));
+  }
+  n_list += 2;
+}
+
 template <bool SMALL = false>
 __device__ __forceinline__ void row_phase_b2_list(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e,
                                                   const RowB1 &r, float cs_cost, float pose_c, int n_list, bool dense) {
-  if (r.fmax > 0.0f) {  // the worst pair's gradient: two more list entries
-    if (lane == 0) {
-      const float4 pi = es.sph[r.bi], pj = es.sph[r.bj];
-      const float w = a.cfg.self_weight;
-      const float gx = w * (pj.x - pi.x), gy = w * (pj.y - pi.y), gz = w * (pj.z - pi.z);
-      es.glist[n_list] = make_float4(gx, gy, gz, __int_as_float(r.bi));
-      es.glist[n_list + 1] = make_float4(-gx, -gy, -gz, __int_as_float(r.bj));
-    }
-    n_list += 2;
+  if (r.fmax > 0.0f) {
+    append_self_pair(a, es, lane, r.bi, r.bj, es.glist, n_list);
     __syncwarp();
   }
   float *gq = a.grad_q + (size_t)e * rv.D;
@@ -683,22 +691,9 @@ __global__ void __launch_bounds__(kBigWarps * 32, 1) rollout_fused_big_kernel(co
     bool dense;
     const RowB1 r = row_phase_b1_list<SCENE, SMALL>(a, rv, es, lane, e, b, n_list, dense);
     row_phase_b2_list<SMALL>(a, rv, es, lane, e, r, cs_cost, pose_c, n_list, dense);
-    if (a.work_counter != nullptr) {
-      int nxt = 0;
-      if (lane == 0) nxt = total_warps + atomicAdd(a.work_counter, 1);
-      e = __shfl_sync(kFull, nxt, 0);
-    } else {
-      e += total_warps;
-    }
+    e = next_warp_unit(a.work_counter, e, total_warps, lane == 0);
   }
-  // the last warp to leave re-arms the counter for the next launch on this stream
-  if (a.work_counter != nullptr && lane == 0) {
-    __threadfence();
-    if (atomicAdd(a.work_counter + 1, 1) == total_warps - 1) {
-      a.work_counter[0] = 0;
-      a.work_counter[1] = 0;
-    }
-  }
+  if (a.work_counter != nullptr && lane == 0) rearm_ticket_counter(a.work_counter, total_warps);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -754,7 +749,7 @@ __global__ void __launch_bounds__(kBigWarps * 32, 1) rollout_fused_team_kernel(c
       tw == 0 ? es.glist : reinterpret_cast<float4 *>(extra + ((TEAM * rv.nl + 24 + 4 * TEAM + 3) & ~3)) + (tw - 1) * kGradListCap;
   const int bar_id = 1 + team;
   const cb200_rollout_cfg &cfg = a.cfg;
-  const int N = a.B * a.H, S = rv.S, D = rv.D, L = rv.L;
+  const int N = a.B * a.H, S = rv.S, D = rv.D;
   const int total_teams = gridDim.x * nteams;
   int e = blockIdx.x * nteams + team;
   while (e < N) {
@@ -765,18 +760,7 @@ __global__ void __launch_bounds__(kBigWarps * 32, 1) rollout_fused_team_kernel(c
     }
     // ---------------- phase A
     if (tw == 0) {
-      float cs = 0.0f;
-#pragma unroll 1
-      for (int d = lane; d < D; d += 32) {
-        const bspline::State4 st = load_row_state<false>(a, e, b, h, d, D);
-        es.qv[d] = st.p;
-        float gp;
-        const float c = cspace_dof(a, rv, e, b, h, d, st, gp);
-        es.gqv[d] = gp;
-        cs += c;
-        if (a.cspace_cost) a.cspace_cost[(size_t)e * D + d] = c;
-      }
-      cs = warp_sum(cs);
+      const float cs = warp_sum(row_cspace<false>(a, rv, es, lane, e, b, h));
       if (lane == 0) ts->cs_cost = cs;
     }
     CB200_NAMED_BARRIER(bar_id, tsize);
@@ -796,7 +780,7 @@ __global__ void __launch_bounds__(kBigWarps * 32, 1) rollout_fused_team_kernel(c
     CB200_NAMED_BARRIER(bar_id, tsize);
     if (tw == 0) warp_fk_compose(rv, es, lane);
     CB200_NAMED_BARRIER(bar_id, tsize);
-    {
+    {  // spheres over the whole team: warp_spheres' vector loads of the link transform took the 2-warp build from 126 to 128 registers
       const float4 *cfg_sph = row_sphere_cfg(a, b, S);
       float4 *out_global = a.robot_spheres ? reinterpret_cast<float4 *>(a.robot_spheres) + (size_t)e * S : nullptr;
 #pragma unroll 1
@@ -808,57 +792,10 @@ __global__ void __launch_bounds__(kBigWarps * 32, 1) rollout_fused_team_kernel(c
         es.sph[s] = w;
         if (out_global != nullptr) out_global[s] = w;
       }
-#pragma unroll 1
-      for (int ca = tlane; ca < rv.n_cl; ca += tsize) {  // link bounds of the self-collision broad phase
-        const float4 c = rv.cl_bound[ca];
-        const float *T = es.cumul + 12 * rv.cl_link[ca];
-        es.bc[ca] = make_float4(T[0] * c.x + T[1] * c.y + T[2] * c.z + T[3], T[4] * c.x + T[5] * c.y + T[6] * c.z + T[7],
-                                T[8] * c.x + T[9] * c.y + T[10] * c.z + T[11], c.w);
-      }
     }
-    if (tw == TEAM - 1) {  // tool poses + tool-pose cost
-      float pose_c = 0.0f;
-      const bool do_pose = (a.goal_position != nullptr);
-#pragma unroll 1
-      for (int t = lane; t < L; t += 32) {
-        const float *T = es.cumul + 12 * rv.tool_map[t];
-        const V3 p = mk3(T[3], T[7], T[11]);
-        const Q4 qt = quat_from_transform(T);
-        if (a.link_pos) {
-          float *o = a.link_pos + ((size_t)e * L + t) * 3;
-          o[0] = p.x;
-          o[1] = p.y;
-          o[2] = p.z;
-        }
-        if (a.link_quat) *reinterpret_cast<float4 *>(a.link_quat + ((size_t)e * L + t) * 4) = make_float4(qt.w, qt.x, qt.y, qt.z);
-        float *pg = es.pose_g + 8 * t;
-        pg[0] = pg[1] = pg[2] = pg[4] = pg[5] = pg[6] = 0.0f;
-        if (do_pose) {
-          const int gi = a.idxs_goal ? __ldg(a.idxs_goal + b) : 0;
-          const bool term = !(h < a.H - 1 && a.H > 1);
-          const float *axes = term ? a.pose_axes_t : a.pose_axes_nt;
-          const float *tol = term ? a.pose_tol_t : a.pose_tol_nt;
-          const size_t go = ((size_t)gi * L + t) * cfg.num_goalset;
-          const PoseOut po = tool_pose_cost(p, qt, a.goal_position + go * 3, a.goal_quat + go * 4, cfg.num_goalset,
-                                            cfg.pose_weight[0], cfg.pose_weight[1], axes, t,
-                                            tol != nullptr ? __ldg(tol + 2 * t) : 0.0f,
-                                            tol != nullptr ? __ldg(tol + 2 * t + 1) : 0.0f, cfg.pose_rotation_method);
-          const V3 om = quat_grad_to_omega(qt, po.gq_w, po.gq_x, po.gq_y, po.gq_z);
-          pg[0] = po.g_pos.x;
-          pg[1] = po.g_pos.y;
-          pg[2] = po.g_pos.z;
-          pg[4] = om.x;
-          pg[5] = om.y;
-          pg[6] = om.z;
-          pose_c += po.pos_cost + po.rot_cost;
-          if (a.pose_cost) {
-            a.pose_cost[((size_t)e * L + t) * 2] = po.pos_cost;
-            a.pose_cost[((size_t)e * L + t) * 2 + 1] = po.rot_cost;
-          }
-          if (a.pose_goalset_idx) a.pose_goalset_idx[(size_t)e * L + t] = po.goal_idx;
-        }
-      }
-      pose_c = warp_sum(pose_c);
+    link_bounds<TEAM * 32>(rv, es, tlane);
+    if (tw == TEAM - 1) {
+      const float pose_c = warp_sum(row_tool_poses(a, rv, es, lane, e, b, h));
       if (lane == 0) ts->pose_c = pose_c;
     }
     CB200_NAMED_BARRIER(bar_id, tsize);
@@ -885,34 +822,10 @@ __global__ void __launch_bounds__(kBigWarps * 32, 1) rollout_fused_team_kernel(c
     if (a.self_cost && tlane == 0) a.self_cost[e] = self_c;
     const bool do_scene = SCENE != 0 && cfg.scene_weight > 0.0f;
     const int env = (a.env_query_idx != nullptr) ? __ldg(a.env_query_idx + b) : 0;
-    int ce = 0, ncub = 0;
-    bool cull = false;
-    if ((SCENE & 1) && do_scene) {
-      ce = env < a.cuboids.num_envs ? env : 0;
-      ncub = a.cuboids.count[ce];
-      if (ncub > a.cuboids.max_n) ncub = a.cuboids.max_n;
-      cull = rv.n_lp > 0 && ncub <= 32;
-      if (cull) {
-#pragma unroll 1
-        for (int ca = tlane; ca < rv.n_cl; ca += tsize) {
-          const float4 cb = rv.cl_bound_scene[ca];
-          uint32_t mask = 0u;
-          if (cb.w >= 0.0f) {
-            const float *Tk = es.cumul + 12 * rv.cl_link[ca];
-            const V3 cw = mk3(Tk[0] * cb.x + Tk[1] * cb.y + Tk[2] * cb.z + Tk[3], Tk[4] * cb.x + Tk[5] * cb.y + Tk[6] * cb.z + Tk[7],
-                              Tk[8] * cb.x + Tk[9] * cb.y + Tk[10] * cb.z + Tk[11]);
-#pragma unroll 1
-            for (int i = 0; i < ncub; ++i) {
-              const int kk = ce * a.cuboids.max_n + i;
-              if (a.cuboids.enable[kk] != 1) continue;
-              const ObsFrame f = load_obs_frame(a.cuboids.inv_pose + 8 * kk);
-              const SdfGrad sg = cuboid_sdf_grad(to_obstacle(f, cw), ldgf(a.cuboids.dims + 4 * kk), ldgf(a.cuboids.dims + 4 * kk + 1),
-                                                 ldgf(a.cuboids.dims + 4 * kk + 2));
-              if (sg.sdf < cb.w + cfg.scene_activation) mask |= (1u << i);
-            }
-          }
-          es.cmask[ca] = mask;
-        }
+    CuboidCull cc{0, 0, false};
+    if (has_cuboids<SCENE>(a, do_scene)) {
+      if (cuboid_cull_state(a, rv, env, true, cc)) {
+        cuboid_cull_masks(a, rv, es, cc.ce, cc.ncub, tlane, tsize);
         CB200_NAMED_BARRIER(bar_id, tsize);
       }
     }
@@ -924,37 +837,7 @@ __global__ void __launch_bounds__(kBigWarps * 32, 1) rollout_fused_team_kernel(c
       const int s = sb + lane;
       V3 g = mk3(0, 0, 0);
       float c = 0.0f;
-      if (s < S && do_scene) {
-        const float4 sp = es.sph[s];
-        const V3 cen = mk3(sp.x, sp.y, sp.z);
-        if (sp.w >= 0.0f) {
-          if (SCENE & 1) {
-            uint32_t m = cull ? es.cmask[rv.sph_cl[s]] : 0xffffffffu;
-            const float radj = sp.w + cfg.scene_activation;
-#pragma unroll 1
-            for (int i = 0; i < ncub && m != 0u; ++i) {
-              if (cull && !((m >> i) & 1u)) continue;
-              if (cull) m &= ~(1u << i);
-              const int kk = ce * a.cuboids.max_n + i;
-              if (a.cuboids.enable[kk] != 1) continue;
-              const ObsFrame f = load_obs_frame(a.cuboids.inv_pose + 8 * kk);
-              const SdfGrad sg = cuboid_sdf_grad(to_obstacle(f, cen), ldgf(a.cuboids.dims + 4 * kk), ldgf(a.cuboids.dims + 4 * kk + 1),
-                                                 ldgf(a.cuboids.dims + 4 * kk + 2));
-              const float pen = radj - sg.sdf;
-              if (pen > 0.0f) {
-                float ac, as;
-                collision_activation(pen, cfg.scene_activation, ac, as);
-                c += cfg.scene_weight * ac;
-                g = g + (cfg.scene_weight * as) * from_obstacle(f, sg.n);
-              }
-            }
-          }
-          if (SCENE & 2) {
-            const CuboidSet none{};
-            c += sphere_scene_discrete<2>(cen, sp.w, cfg.scene_activation, cfg.scene_weight, none, a.voxels, env, g);
-          }
-        }
-      }
+      if (s < S && do_scene) c = sphere_discrete_terms<SCENE>(a, rv, es, cc, env, s, g);
       const bool nz = (g.x != 0.0f) || (g.y != 0.0f) || (g.z != 0.0f);
       const unsigned m = __ballot_sync(kFull, nz);
       if (m) {
@@ -974,16 +857,7 @@ __global__ void __launch_bounds__(kBigWarps * 32, 1) rollout_fused_team_kernel(c
     if (lane == 0) ts->scene_c[tw] = scene_c;
     {
       // ---------------- phase B2: J^T over the team's list segments
-      if (tw == 0 && fmax > 0.0f) {
-        if (lane == 0) {
-          const float4 pi = es.sph[bi], pj = es.sph[bj];
-          const float w = cfg.self_weight;
-          const float gx = w * (pj.x - pi.x), gy = w * (pj.y - pi.y), gz = w * (pj.z - pi.z);
-          my_list[n_list] = make_float4(gx, gy, gz, __int_as_float(bi));
-          my_list[n_list + 1] = make_float4(-gx, -gy, -gz, __int_as_float(bj));
-        }
-        n_list += 2;
-      }
+      if (tw == 0 && fmax > 0.0f) append_self_pair(a, es, lane, bi, bj, my_list, n_list);
       __syncwarp();  // the warp's list entries are visible to all of its lanes
       float acc[2];
       warp_list_accumulate(rv, es, lane, my_list, n_list, tw == 0, acc);
@@ -1023,14 +897,7 @@ __global__ void __launch_bounds__(kBigWarps * 32, 1) rollout_fused_team_kernel(c
     e = ts->next_row;
     CB200_NAMED_BARRIER(bar_id, tsize);  // every warp has read next_row / the row state before the next row rewrites them
   }
-  // the last team to leave re-arms the counter for the next launch
-  if (a.work_counter != nullptr && tw == 0 && lane == 0) {
-    __threadfence();
-    if (atomicAdd(a.work_counter + 1, 1) == total_teams - 1) {
-      a.work_counter[0] = 0;
-      a.work_counter[1] = 0;
-    }
-  }
+  if (a.work_counter != nullptr && tw == 0 && lane == 0) rearm_ticket_counter(a.work_counter, total_teams);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1039,6 +906,45 @@ __global__ void __launch_bounds__(kBigWarps * 32, 1) rollout_fused_team_kernel(c
 // waypoint (warp 0 / the last warp also compute the halo waypoints' spheres), the CTA synchronises, then
 // every warp runs phase B reading its neighbours' sphere positions from shared memory.
 // ------------------------------------------------------------------------------------------------
+// Halo waypoints of the tile h0 .. h0 + nwarps - 1 of seed b, spheres only: warp 0 writes those of h0 - 1 to halo_prev, the last
+// warp those of h0 + nwarps to halo_next (when the trajectory has them).  Uses the warp's row state as scratch.
+template <bool SPLINE>
+__device__ __forceinline__ void tile_halo(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int warp, int nwarps,
+                                          int b, int h0, float4 *halo_prev, float4 *halo_next) {
+  const int D = rv.D, S = rv.S;
+  int hh = -1;
+  float4 *hdst = nullptr;
+  if (warp == 0 && h0 > 0) {
+    hh = h0 - 1;
+    hdst = halo_prev;
+  } else if (warp == nwarps - 1 && h0 + nwarps < a.H) {
+    hh = h0 + nwarps;
+    hdst = halo_next;
+  }
+  if (hh >= 0) {
+    const size_t eh = (size_t)b * a.H + hh;
+    for (int d = lane; d < D; d += 32)
+      es.qv[d] = SPLINE ? spline_row_state(a.spl, b, hh, d, D).p : __ldg(a.q + eh * D + d);
+    __syncwarp();
+    warp_fk(rv, es, lane);
+    const float4 *cfg_sph = row_sphere_cfg(a, b, S);
+    for (int s = lane; s < S; s += 32) {
+      const float *T = es.cumul + 12 * rv.sph_link[s];
+      const float4 p = cfg_sph != nullptr ? __ldg(cfg_sph + s) : rv.spheres[s];
+      hdst[s] = make_float4(T[0] * p.x + T[1] * p.y + T[2] * p.z + T[3], T[4] * p.x + T[5] * p.y + T[6] * p.z + T[7],
+                            T[8] * p.x + T[9] * p.y + T[10] * p.z + T[11], p.w);
+    }
+    __syncwarp();
+  }
+}
+
+// Spheres of a neighbouring waypoint for the swept terms: those of warp nb's row when nb is in the tile (`all` holds the warps'
+// eval_floats slices), else the halo
+__device__ __forceinline__ const float4 *neighbour_spheres(const FusedArgs &a, const RobotView &rv, const float *all, int nb, bool in_tile,
+                                                          const float4 *halo) {
+  return in_tile ? reinterpret_cast<const float4 *>(all + (size_t)nb * a.eval_floats + rv.nl * 12) : halo;
+}
+
 // SMALL: arms (<= 24 links, <= 128 spheres): whole-block self-collision scan and the one-slot sparse J^T (see the IK arm build).
 template <int SCENE, bool SPLINE, bool SMALL = false>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, kMinCtas) rollout_traj_kernel(const __grid_constant__ FusedArgs a) {
@@ -1051,7 +957,6 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kMinCtas) rollout_traj_kern
   const EvalSmem es = carve_eval_smem(all + (size_t)warp * a.eval_floats, rv.nl, rv.D, rv.S, rv.L, rv.n_cl);
   float4 *halo_prev = reinterpret_cast<float4 *>(all + (size_t)nwarps * a.eval_floats);
   float4 *halo_next = halo_prev + rv.S;
-  const int D = rv.D, S = rv.S;
   const int tiles_per_seed = (a.H + nwarps - 1) / nwarps;
   const long long n_tiles = (long long)a.B * tiles_per_seed;
   __shared__ int next_tile;  // tiles after a CTA's first come from the ticket counter (tiles differ in cost: see rollout_fused_kernel)
@@ -1060,31 +965,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kMinCtas) rollout_traj_kern
     const int h0 = (int)(tile - (long long)b * tiles_per_seed) * nwarps;
     const int h = h0 + warp;
     const bool active = h < a.H;
-    // halo waypoints: spheres only
-    int hh = -1;
-    float4 *hdst = nullptr;
-    if (warp == 0 && h0 > 0) {
-      hh = h0 - 1;
-      hdst = halo_prev;
-    } else if (warp == nwarps - 1 && h0 + nwarps < a.H) {
-      hh = h0 + nwarps;
-      hdst = halo_next;
-    }
-    if (hh >= 0) {
-      const size_t eh = (size_t)b * a.H + hh;
-      for (int d = lane; d < D; d += 32)
-        es.qv[d] = SPLINE ? spline_row_state(a.spl, b, hh, d, D).p : __ldg(a.q + eh * D + d);
-      __syncwarp();
-      warp_fk(rv, es, lane);
-      const float4 *cfg_sph = row_sphere_cfg(a, b, S);
-      for (int s = lane; s < S; s += 32) {
-        const float *T = es.cumul + 12 * rv.sph_link[s];
-        const float4 p = cfg_sph != nullptr ? __ldg(cfg_sph + s) : rv.spheres[s];
-        hdst[s] = make_float4(T[0] * p.x + T[1] * p.y + T[2] * p.z + T[3], T[4] * p.x + T[5] * p.y + T[6] * p.z + T[7],
-                              T[8] * p.x + T[9] * p.y + T[10] * p.z + T[11], p.w);
-      }
-      __syncwarp();
-    }
+    tile_halo<SPLINE>(a, rv, es, lane, warp, nwarps, b, h0, halo_prev, halo_next);
     const int e = b * a.H + h;
     float cs_cost = 0.0f, pose_c = 0.0f;
     RowB1 r{0.0f, 0.0f, 0.0f, 0, 0, 0};
@@ -1092,8 +973,8 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kMinCtas) rollout_traj_kern
     __syncthreads();
     if (active) {
       const float4 *prev = nullptr, *next = nullptr;
-      if (h > 0) prev = (warp > 0) ? reinterpret_cast<const float4 *>(all + (size_t)(warp - 1) * a.eval_floats + rv.nl * 12) : halo_prev;
-      if (h < a.H - 1) next = (warp < nwarps - 1) ? reinterpret_cast<const float4 *>(all + (size_t)(warp + 1) * a.eval_floats + rv.nl * 12) : halo_next;
+      if (h > 0) prev = neighbour_spheres(a, rv, all, warp - 1, warp > 0, halo_prev);
+      if (h < a.H - 1) next = neighbour_spheres(a, rv, all, warp + 1, warp < nwarps - 1, halo_next);
       r = row_phase_b1<true, SCENE, !SMALL>(a, rv, es, lane, e, b, prev, next);
     }
     if (threadIdx.x == 0 && a.work_counter != nullptr) next_tile = (int)gridDim.x + atomicAdd(a.work_counter, 1);
@@ -1102,13 +983,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kMinCtas) rollout_traj_kern
     // (next_tile is rewritten only after the next iteration's first __syncthreads, which every thread passes after this read)
     tile = a.work_counter != nullptr ? (long long)next_tile : tile + gridDim.x;
   }
-  if (a.work_counter != nullptr && threadIdx.x == 0) {  // the last CTA to leave re-arms the counter for the next launch
-    __threadfence();
-    if (atomicAdd(a.work_counter + 1, 1) == (int)gridDim.x - 1) {
-      a.work_counter[0] = 0;
-      a.work_counter[1] = 0;
-    }
-  }
+  if (a.work_counter != nullptr && threadIdx.x == 0) rearm_ticket_counter(a.work_counter, (int)gridDim.x);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1200,29 +1075,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kMinCtas) rollout_traj_dyn_
       const int h0 = c0 + t0;
       const int h = h0 + warp;
       const bool active = h < a.H;
-      int hh = -1;
-      float4 *hdst = nullptr;
-      if (warp == 0 && h0 > 0) {
-        hh = h0 - 1;
-        hdst = halo_prev;
-      } else if (warp == nwarps - 1 && h0 + nwarps < a.H) {
-        hh = h0 + nwarps;
-        hdst = halo_next;
-      }
-      if (hh >= 0) {
-        const size_t eh = (size_t)b * a.H + hh;
-        for (int d = lane; d < D; d += 32) es.qv[d] = __ldg(a.q + eh * D + d);
-        __syncwarp();
-        warp_fk(rv, es, lane);
-        const float4 *cfg_sph = row_sphere_cfg(a, b, S);
-        for (int s = lane; s < S; s += 32) {
-          const float *Tm = es.cumul + 12 * rv.sph_link[s];
-          const float4 p = cfg_sph != nullptr ? __ldg(cfg_sph + s) : rv.spheres[s];
-          hdst[s] = make_float4(Tm[0] * p.x + Tm[1] * p.y + Tm[2] * p.z + Tm[3], Tm[4] * p.x + Tm[5] * p.y + Tm[6] * p.z + Tm[7],
-                                Tm[8] * p.x + Tm[9] * p.y + Tm[10] * p.z + Tm[11], p.w);
-        }
-        __syncwarp();
-      }
+      tile_halo<false>(a, rv, es, lane, warp, nwarps, b, h0, halo_prev, halo_next);
       const int e = b * a.H + h;
       float cs_cost = 0.0f, pose_c = 0.0f;
       RowB1 r{0.0f, 0.0f, 0.0f, 0, 0, 0};
@@ -1244,8 +1097,8 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, kMinCtas) rollout_traj_dyn_
       __syncthreads();
       if (active) {
         const float4 *prev = nullptr, *next = nullptr;
-        if (h > 0) prev = (warp > 0) ? reinterpret_cast<const float4 *>(all + (size_t)(warp - 1) * a.eval_floats + rv.nl * 12) : halo_prev;
-        if (h < a.H - 1) next = (warp < nwarps - 1) ? reinterpret_cast<const float4 *>(all + (size_t)(warp + 1) * a.eval_floats + rv.nl * 12) : halo_next;
+        if (h > 0) prev = neighbour_spheres(a, rv, all, warp - 1, warp > 0, halo_prev);
+        if (h < a.H - 1) next = neighbour_spheres(a, rv, all, warp + 1, warp < nwarps - 1, halo_next);
         r = row_phase_b1<true, SCENE>(a, rv, es, lane, e, b, prev, next);
       }
       __syncthreads();

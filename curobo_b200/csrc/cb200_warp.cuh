@@ -378,6 +378,19 @@ __device__ __forceinline__ float warp_self_collision_pairs(const float4 *psph, c
 // with lanes over the flattened |a| x |b| tile.
 // ----------------------------------------------------------------------------------------------
 // PADDED_COPY = false (big-robot layout): the padded sphere is rebuilt from the world sphere + the padding table on every read.
+// World-frame bounding sphere of every collision link (es.bc), over the W lanes of a row, or of a team of warps sharing one
+// (W = TEAM x 32, `lane` = the lane within the team).
+template <int W = 32>
+__device__ __forceinline__ void link_bounds(const RobotView &rv, const EvalSmem &es, int lane) {
+  #pragma unroll 1
+  for (int a = lane; a < rv.n_cl; a += W) {
+    const float4 c = rv.cl_bound[a];
+    const float *T = es.cumul + 12 * rv.cl_link[a];
+    es.bc[a] = make_float4(T[0] * c.x + T[1] * c.y + T[2] * c.z + T[3], T[4] * c.x + T[5] * c.y + T[6] * c.z + T[7],
+                           T[8] * c.x + T[9] * c.y + T[10] * c.z + T[11], c.w);
+  }
+}
+
 template <bool PADDED_COPY>
 __device__ __forceinline__ float4 padded_sphere(const RobotView &rv, const EvalSmem &es, int i) {
   if (PADDED_COPY) return es.gsph[i];
@@ -398,13 +411,7 @@ __device__ __forceinline__ float warp_self_collision_tiles(const RobotView &rv, 
                                                            unsigned long long *key_out = nullptr, bool fill_bounds = true) {
   static_assert(W == 32 || !CULL2, "the second-level cull is written for whole-warp rows");
   if (fill_bounds) {
-    #pragma unroll 1
-    for (int a = lane; a < rv.n_cl; a += W) {
-      const float4 c = rv.cl_bound[a];
-      const float *T = es.cumul + 12 * rv.cl_link[a];
-      es.bc[a] = make_float4(T[0] * c.x + T[1] * c.y + T[2] * c.z + T[3], T[4] * c.x + T[5] * c.y + T[6] * c.z + T[7],
-                             T[8] * c.x + T[9] * c.y + T[10] * c.z + T[11], c.w);
-    }
+    link_bounds<W>(rv, es, lane);
     row_sync<W>();
   }
   unsigned long long key = 0ull;  // f bits | ~i | ~j : max = largest f, then smallest i, then smallest j
