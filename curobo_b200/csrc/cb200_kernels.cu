@@ -153,7 +153,8 @@ __device__ __forceinline__ float seed_dt(const FusedArgs &a, int b) {
   return a.dt ? __ldg(a.dt + b) : 1.0f;
 }
 
-// c-space cost for one dof; returns cost, writes gradient wrt position into gp (and v/a/j grads to global)
+// c-space cost for one dof; returns cost, writes gradient wrt position into gp (and v/a/j grads to global unless !GRAD)
+template <bool GRAD = true>
 __device__ __forceinline__ float cspace_dof(const FusedArgs &a, const RobotView &rv, int e, int b, int h, int d,
                                             const bspline::State4 &st, float &gp) {
   const float qd = st.p;
@@ -199,9 +200,11 @@ __device__ __forceinline__ float cspace_dof(const FusedArgs &a, const RobotView 
     l2_reg(v, wr[0], cost, gv);
     l2_reg(ac, wr[1], cost, ga);
     l2_reg(jk, wr[2], cost, gj);
-    if (a.grad_vel) a.grad_vel[idx] = gv;
-    if (a.grad_acc) a.grad_acc[idx] = ga;
-    if (a.grad_jerk) a.grad_jerk[idx] = gj;
+    if (GRAD) {
+      if (a.grad_vel) a.grad_vel[idx] = gv;
+      if (a.grad_acc) a.grad_acc[idx] = ga;
+      if (a.grad_jerk) a.grad_jerk[idx] = gj;
+    }
   }
   return cost;
 }
@@ -211,10 +214,12 @@ __device__ __forceinline__ float cspace_dof(const FusedArgs &a, const RobotView 
 //   phase A: q load + c-space cost, FK, spheres (+ padded copy), tool poses + tool-pose cost
 //   phase B: self collision, scene collision (discrete | swept + speed metric), J^T backward, row cost
 // The helpers are inlined: out-of-line phases needed fewer registers and ran slower (DESIGN.md section 4).
+// GRAD = false (the cost-only kernels): the same costs, minus everything whose only consumer is the gradient -- the c-space and
+// pose gradients, the sphere gradients and their count, the self-collision pair gradient, the J^T backward.
 // ------------------------------------------------------------------------------------------------
 
 // c-space phase of row (b, h): loads the row state into es.qv, the position gradient into es.gqv; returns the lane's cost sum
-template <bool SPLINE, int W = 32>
+template <bool SPLINE, int W = 32, bool GRAD = true>
 __device__ __forceinline__ float row_cspace(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e, int b,
                                             int h) {
   const int D = rv.D;
@@ -224,8 +229,8 @@ __device__ __forceinline__ float row_cspace(const FusedArgs &a, const RobotView 
     const bspline::State4 st = load_row_state<SPLINE>(a, e, b, h, d, D);
     es.qv[d] = st.p;
     float gp;
-    const float c = cspace_dof(a, rv, e, b, h, d, st, gp);
-    es.gqv[d] = gp;
+    const float c = cspace_dof<GRAD>(a, rv, e, b, h, d, st, gp);
+    if (GRAD) es.gqv[d] = gp;
     cs_cost += c;
     if (a.cspace_cost) a.cspace_cost[(size_t)e * D + d] = c;
   }
@@ -234,7 +239,7 @@ __device__ __forceinline__ float row_cspace(const FusedArgs &a, const RobotView 
 
 // tool poses of row (b, h) (link_pos / link_quat) and the tool-pose cost: its gradient goes to es.pose_g; returns the lane's
 // cost sum
-template <int W = 32>
+template <int W = 32, bool GRAD = true>
 __device__ __forceinline__ float row_tool_poses(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e, int b,
                                                 int h) {
   const cb200_rollout_cfg &cfg = a.cfg;
@@ -253,8 +258,8 @@ __device__ __forceinline__ float row_tool_poses(const FusedArgs &a, const RobotV
       o[2] = p.z;
     }
     if (a.link_quat) *reinterpret_cast<float4 *>(a.link_quat + ((size_t)e * L + t) * 4) = make_float4(qt.w, qt.x, qt.y, qt.z);
-    float *pg = es.pose_g + 8 * t;
-    pg[0] = pg[1] = pg[2] = pg[4] = pg[5] = pg[6] = 0.0f;
+    float *pg = GRAD ? es.pose_g + 8 * t : nullptr;
+    if (GRAD) pg[0] = pg[1] = pg[2] = pg[4] = pg[5] = pg[6] = 0.0f;
     if (do_pose) {
       const int gi = a.idxs_goal ? __ldg(a.idxs_goal + b) : 0;
       const bool term = !(h < a.H - 1 && a.H > 1);
@@ -265,13 +270,15 @@ __device__ __forceinline__ float row_tool_poses(const FusedArgs &a, const RobotV
                                         cfg.pose_weight[0], cfg.pose_weight[1], axes, t,
                                         tol != nullptr ? __ldg(tol + 2 * t) : 0.0f,
                                         tol != nullptr ? __ldg(tol + 2 * t + 1) : 0.0f, cfg.pose_rotation_method);
-      const V3 om = quat_grad_to_omega(qt, po.gq_w, po.gq_x, po.gq_y, po.gq_z);
-      pg[0] = po.g_pos.x;
-      pg[1] = po.g_pos.y;
-      pg[2] = po.g_pos.z;
-      pg[4] = om.x;
-      pg[5] = om.y;
-      pg[6] = om.z;
+      if (GRAD) {
+        const V3 om = quat_grad_to_omega(qt, po.gq_w, po.gq_x, po.gq_y, po.gq_z);
+        pg[0] = po.g_pos.x;
+        pg[1] = po.g_pos.y;
+        pg[2] = po.g_pos.z;
+        pg[4] = om.x;
+        pg[5] = om.y;
+        pg[6] = om.z;
+      }
       pose_c += po.pos_cost + po.rot_cost;
       if (a.pose_cost) {
         a.pose_cost[((size_t)e * L + t) * 2] = po.pos_cost;
@@ -283,16 +290,16 @@ __device__ __forceinline__ float row_tool_poses(const FusedArgs &a, const RobotV
   return pose_c;
 }
 
-template <bool SPLINE, int W = 32>
+template <bool SPLINE, int W = 32, bool GRAD = true>
 __device__ __forceinline__ void row_phase_a(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e,
                                             int b, int h, float &cs_cost, float &pose_c) {
   const int S = rv.S;
-  cs_cost = row_cspace<SPLINE, W>(a, rv, es, lane, e, b, h);
+  cs_cost = row_cspace<SPLINE, W, GRAD>(a, rv, es, lane, e, b, h);
   row_sync<W>();
   warp_fk<W>(rv, es, lane);
   warp_spheres<W>(rv, es, lane, a.robot_spheres ? reinterpret_cast<float4 *>(a.robot_spheres) + (size_t)e * S : nullptr,
                   row_sphere_cfg(a, b, S));
-  pose_c = row_tool_poses<W>(a, rv, es, lane, e, b, h);
+  pose_c = row_tool_poses<W, GRAD>(a, rv, es, lane, e, b, h);
   row_sync<W>();
 }
 
@@ -409,15 +416,15 @@ __device__ __forceinline__ float sphere_discrete_terms(const FusedArgs &a, const
   return c;
 }
 
-template <bool SWEEP, int SCENE, bool CULL2 = true, int W = 32>
+template <bool SWEEP, int SCENE, bool CULL2 = true, int W = 32, bool GRAD = true>
 __device__ __forceinline__ RowB1 row_phase_b1(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e,
                                               int b, const float4 *prev_sph, const float4 *next_sph) {
   const cb200_rollout_cfg &cfg = a.cfg;
   const int S = rv.S;
   RowB1 r{0.0f, 0.0f, 0.0f, 0, 0, 0};
-  // ---- self collision (reads padded spheres in gsph)
+  // ---- self collision (reads padded spheres in gsph; the cost-only layout keeps that copy only for the pair scan)
   if (cfg.self_weight > 0.0f && rv.P > 0) {
-    r.fmax = (rv.n_lp > 0) ? warp_self_collision_tiles<true, CULL2, W>(rv, es, lane, r.bi, r.bj)
+    r.fmax = (rv.n_lp > 0) ? warp_self_collision_tiles<GRAD, CULL2, W>(rv, es, lane, r.bi, r.bj)
                            : warp_self_collision_pairs<W>(es.gsph, rv.pairs, rv.P, lane, r.bi, r.bj);
     r.self_c = (r.fmax > 0.0f) ? 0.5f * cfg.self_weight * r.fmax : 0.0f;
   }
@@ -466,38 +473,42 @@ __device__ __forceinline__ RowB1 row_phase_b1(const FusedArgs &a, const RobotVie
         if (cfg.use_speed_metric && prev_sph != nullptr && next_sph != nullptr) speed_metric(pv, cen, nx, sdt, c, g);
       }
     }
-    es.gsph[s] = make_float4(g.x, g.y, g.z, 0.0f);
-    r.nnz += (g.x != 0.0f || g.y != 0.0f || g.z != 0.0f) ? 1 : 0;
+    if (GRAD) {
+      es.gsph[s] = make_float4(g.x, g.y, g.z, 0.0f);
+      r.nnz += (g.x != 0.0f || g.y != 0.0f || g.z != 0.0f) ? 1 : 0;
+    }
     r.scene_c += c;
     if (a.scene_cost) a.scene_cost[(size_t)e * S + s] = c;
   }
   row_sync<W>();
-  r.nnz = (int)row_reduce<W, 0>((unsigned)r.nnz) + 2;  // + the two self-collision spheres
+  if (GRAD) r.nnz = (int)row_reduce<W, 0>((unsigned)r.nnz) + 2;  // + the two self-collision spheres
   return r;
 }
 
 // phase B2: add the self-collision gradient to the two spheres of the worst pair, J^T backward, row cost.
-template <bool SMALL = false, int W = 32>
+template <bool SMALL = false, int W = 32, bool GRAD = true>
 __device__ __forceinline__ void row_phase_b2(const FusedArgs &a, const RobotView &rv, const EvalSmem &es,
                                              const unsigned char *smem_blob, int lane, int e, const RowB1 &r,
                                              float cs_cost, float pose_c) {
-  if (r.fmax > 0.0f && lane == 0) {
-    const float4 pi = es.sph[r.bi], pj = es.sph[r.bj];
-    const float w = a.cfg.self_weight;
-    float4 gi = es.gsph[r.bi], gj = es.gsph[r.bj];
-    const float gx = w * (pj.x - pi.x), gy = w * (pj.y - pi.y), gz = w * (pj.z - pi.z);
-    gi.x += gx;
-    gi.y += gy;
-    gi.z += gz;
-    gj.x -= gx;
-    gj.y -= gy;
-    gj.z -= gz;
-    es.gsph[r.bi] = gi;
-    es.gsph[r.bj] = gj;
+  if (GRAD) {
+    if (r.fmax > 0.0f && lane == 0) {
+      const float4 pi = es.sph[r.bi], pj = es.sph[r.bj];
+      const float w = a.cfg.self_weight;
+      float4 gi = es.gsph[r.bi], gj = es.gsph[r.bj];
+      const float gx = w * (pj.x - pi.x), gy = w * (pj.y - pi.y), gz = w * (pj.z - pi.z);
+      gi.x += gx;
+      gi.y += gy;
+      gi.z += gz;
+      gj.x -= gx;
+      gj.y -= gy;
+      gj.z -= gz;
+      es.gsph[r.bi] = gi;
+      es.gsph[r.bj] = gj;
+    }
+    row_sync<W>();
+    float *gq = a.grad_q + (size_t)e * rv.D;
+    if (!warp_fk_backward_sparse<SMALL, W>(rv, es, lane, gq, r.nnz)) warp_fk_backward_cold<W>(smem_blob, a.blob, es.cumul, lane, gq);
   }
-  row_sync<W>();
-  float *gq = a.grad_q + (size_t)e * rv.D;
-  if (!warp_fk_backward_sparse<SMALL, W>(rv, es, lane, gq, r.nnz)) warp_fk_backward_cold<W>(smem_blob, a.blob, es.cumul, lane, gq);
   const float tot = warp_sum<W>(cs_cost + pose_c + r.scene_c) + r.self_c;
   if (lane == 0) a.cost[e] = tot;
   row_sync<W>();
@@ -565,6 +576,43 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB) rollout_fused_kernel(
   if (a.work_counter != nullptr && leader) rearm_ticket_counter(a.work_counter, stride);
 }
 
+// Cost-only twin of rollout_fused_kernel (cb200_rollout_cost): the same rows and costs through the same phases at GRAD = false,
+// no gradient, a smaller row state (carve_cost_smem).  Discrete rows from caller-provided positions only.  (A body shared with
+// rollout_fused_kernel through one inlined template changed that kernel's register allocation, so the two are kept apart.)
+template <int SCENE, int MINB = kMinCtas, int ROWS = 1>
+__global__ void __launch_bounds__(kWarpsPerCta * 32, MINB) rollout_cost_kernel(const __grid_constant__ FusedArgs a) {
+  static_assert(ROWS == 1 || (ROWS == 2 && MINB == 3), "paired rows: arm build only");
+  constexpr int W = 32 / ROWS;
+  CB200_EXTERN_SHARED __align__(128) unsigned char smem[];
+  __shared__ unsigned long long mbar;
+  stage_blob_to_smem(smem, a.blob, (uint32_t)a.blob_smem_bytes, &mbar);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & (W - 1), nwarps = blockDim.x >> 5;
+  const int half = ROWS == 1 ? 0 : (int)(threadIdx.x >> 4) & 1;
+  const bool leader = (threadIdx.x & 31) == 0;
+  float *base = reinterpret_cast<float *>(smem + a.blob_smem_bytes) + (size_t)(warp * ROWS + half) * a.eval_floats;
+  const int N = a.B * a.H;
+  const int stride = gridDim.x * nwarps;
+  int u = blockIdx.x * nwarps + warp;
+  while (u * ROWS < N) {
+    const int e = u * ROWS + half;
+    if (ROWS == 1 || e < N) {
+      int b = e, h = 0;
+      if (a.H != 1) {
+        b = e / a.H;
+        h = e - b * a.H;
+      }
+      const RobotView rv = make_robot_view(smem, a.blob);
+      const EvalSmem es = carve_cost_smem(base, rv.nl, rv.D, rv.S, rv.n_cl, rv.n_lp == 0);
+      float cs_cost = 0.0f, pose_c = 0.0f;
+      row_phase_a<false, W, false>(a, rv, es, lane, e, b, h, cs_cost, pose_c);
+      const RowB1 r = row_phase_b1<false, SCENE, MINB != 3, W, false>(a, rv, es, lane, e, b, nullptr, nullptr);
+      row_phase_b2<MINB == 3, W, false>(a, rv, es, smem, lane, e, r, cs_cost, pose_c);
+    }
+    u = next_warp_unit(a.work_counter, u, stride, leader);
+  }
+  if (a.work_counter != nullptr && leader) rearm_ticket_counter(a.work_counter, stride);
+}
+
 // ------------------------------------------------------------------------------------------------
 // THE fused kernel for big robots (humanoids), discrete scene collision.  Same phases and arithmetic as rollout_fused_kernel;
 // what changes is how many rows an SM keeps in flight.  The kernel is latency bound and shared memory caps the resident warps: a G1-29 row is 17.3 KB, of which 12.8 KB
@@ -578,7 +626,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB) rollout_fused_kernel(
 // ------------------------------------------------------------------------------------------------
 constexpr int kBigWarps = 16;
 
-template <int SCENE, bool SMALL = false>
+template <int SCENE, bool SMALL = false, bool GRAD = true>
 __device__ __forceinline__ RowB1 row_phase_b1_list(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e,
                                                    int b, int &n_list, bool &dense) {
   const cb200_rollout_cfg &cfg = a.cfg;
@@ -609,27 +657,29 @@ __device__ __forceinline__ RowB1 row_phase_b1_list(const FusedArgs &a, const Rob
     V3 g = mk3(0, 0, 0);
     float c = 0.0f;
     if (s < S && do_scene) c = sphere_discrete_terms<SCENE>(a, rv, es, cc, env, s, g);
-    const bool nz = (g.x != 0.0f) || (g.y != 0.0f) || (g.z != 0.0f);
-    const unsigned m = __ballot_sync(kFull, nz);
-    if (m) {
-      const int cnt = __popc(m);
-      if (n_list + cnt > kGradListCap - 2) {  // (two slots stay free for the self-collision pair)
-        if (!ft_live) {
-          warp_zero_ft(rv, es, lane);
-          ft_live = true;
+    if (GRAD) {
+      const bool nz = (g.x != 0.0f) || (g.y != 0.0f) || (g.z != 0.0f);
+      const unsigned m = __ballot_sync(kFull, nz);
+      if (m) {
+        const int cnt = __popc(m);
+        if (n_list + cnt > kGradListCap - 2) {  // (two slots stay free for the self-collision pair)
+          if (!ft_live) {
+            warp_zero_ft(rv, es, lane);
+            ft_live = true;
+          }
+          warp_drain_list_to_ft(rv, es, lane, n_list);
+          n_list = 0;
+          dense = true;
         }
-        warp_drain_list_to_ft(rv, es, lane, n_list);
-        n_list = 0;
-        dense = true;
+        if (nz) es.glist[n_list + __popc(m & lt)] = make_float4(g.x, g.y, g.z, __int_as_float(s));
+        n_list += cnt;
+        __syncwarp();
       }
-      if (nz) es.glist[n_list + __popc(m & lt)] = make_float4(g.x, g.y, g.z, __int_as_float(s));
-      n_list += cnt;
-      __syncwarp();
     }
     r.scene_c += c;
     if (a.scene_cost && s < S) a.scene_cost[(size_t)e * S + s] = c;
   }
-  if (dense && !ft_live) warp_zero_ft(rv, es, lane);
+  if (GRAD && dense && !ft_live) warp_zero_ft(rv, es, lane);
   return r;
 }
 
@@ -646,19 +696,21 @@ __device__ __forceinline__ void append_self_pair(const FusedArgs &a, const EvalS
   n_list += 2;
 }
 
-template <bool SMALL = false>
+template <bool SMALL = false, bool GRAD = true>
 __device__ __forceinline__ void row_phase_b2_list(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e,
                                                   const RowB1 &r, float cs_cost, float pose_c, int n_list, bool dense) {
-  if (r.fmax > 0.0f) {
-    append_self_pair(a, es, lane, r.bi, r.bj, es.glist, n_list);
-    __syncwarp();
-  }
-  float *gq = a.grad_q + (size_t)e * rv.D;
-  if (!dense) {
-    warp_fk_backward_list<SMALL>(rv, es, lane, gq, n_list);
-  } else {
-    warp_drain_list_to_ft(rv, es, lane, n_list);
-    warp_fk_backward_from_ft(rv, es, lane, gq);
+  if (GRAD) {
+    if (r.fmax > 0.0f) {
+      append_self_pair(a, es, lane, r.bi, r.bj, es.glist, n_list);
+      __syncwarp();
+    }
+    float *gq = a.grad_q + (size_t)e * rv.D;
+    if (!dense) {
+      warp_fk_backward_list<SMALL>(rv, es, lane, gq, n_list);
+    } else {
+      warp_drain_list_to_ft(rv, es, lane, n_list);
+      warp_fk_backward_from_ft(rv, es, lane, gq);
+    }
   }
   const float tot = warp_sum(cs_cost + pose_c + r.scene_c) + r.self_c;
   if (lane == 0) a.cost[e] = tot;
@@ -691,6 +743,37 @@ __global__ void __launch_bounds__(kBigWarps * 32, 1) rollout_fused_big_kernel(co
     bool dense;
     const RowB1 r = row_phase_b1_list<SCENE, SMALL>(a, rv, es, lane, e, b, n_list, dense);
     row_phase_b2_list<SMALL>(a, rv, es, lane, e, r, cs_cost, pose_c, n_list, dense);
+    e = next_warp_unit(a.work_counter, e, total_warps, lane == 0);
+  }
+  if (a.work_counter != nullptr && lane == 0) rearm_ticket_counter(a.work_counter, total_warps);
+}
+
+// Cost-only twin of rollout_fused_big_kernel (cb200_rollout_cost).  Also where cost-only batches go whose gradient launch would
+// take the team kernel: particle batches are large, so there is no cost-only team build.
+template <int SCENE, bool SMALL = false>
+__global__ void __launch_bounds__(kBigWarps * 32, 1) rollout_cost_big_kernel(const __grid_constant__ FusedArgs a) {
+  CB200_EXTERN_SHARED __align__(128) unsigned char smem[];
+  __shared__ unsigned long long mbar;
+  stage_blob_to_smem(smem, a.blob, (uint32_t)a.blob_smem_bytes, &mbar);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+  float *base = reinterpret_cast<float *>(smem + a.blob_smem_bytes) + (size_t)warp * a.eval_floats;
+  const RobotView rv = make_robot_view(smem, a.blob);
+  const EvalSmem es = carve_cost_smem(base, rv.nl, rv.D, rv.S, rv.n_cl, rv.n_lp == 0);
+  const int N = a.B * a.H;
+  const int total_warps = gridDim.x * nwarps;
+  int e = blockIdx.x * nwarps + warp;
+  while (e < N) {
+    int b = e, h = 0;
+    if (a.H != 1) {
+      b = e / a.H;
+      h = e - b * a.H;
+    }
+    float cs_cost = 0.0f, pose_c = 0.0f;
+    row_phase_a<false, 32, false>(a, rv, es, lane, e, b, h, cs_cost, pose_c);
+    int n_list;
+    bool dense;
+    const RowB1 r = row_phase_b1_list<SCENE, SMALL, false>(a, rv, es, lane, e, b, n_list, dense);
+    row_phase_b2_list<SMALL, false>(a, rv, es, lane, e, r, cs_cost, pose_c, n_list, dense);
     e = next_warp_unit(a.work_counter, e, total_warps, lane == 0);
   }
   if (a.work_counter != nullptr && lane == 0) rearm_ticket_counter(a.work_counter, total_warps);
@@ -1962,7 +2045,7 @@ static void bounding_ball(const float *link_spheres, const float *padding, int s
   out[3] = (float)(std::max(Rf, Rr) * (1.0 + 1e-4) + 1e-5);
 }
 
-// which kernel the last cb200_rollout_cost_grad call of this thread launched (CB200_VARIANT_*; test / bench introspection)
+// which kernel the last cb200_rollout_cost_grad / cb200_rollout_cost call of this thread launched (CB200_VARIANT_*; test / bench introspection)
 static thread_local int g_last_variant = 0;
 
 extern "C" {
@@ -2449,10 +2532,17 @@ int64_t cb200_pack_robot_blob(void *out, int64_t out_bytes, const cb200_robot_si
   return total;
 }
 
-int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io *io, cb200_stream_t stream) {
+}  // extern "C"
+
+// cb200_rollout_cost_grad (grad) and cb200_rollout_cost (!grad): one launcher, one kernel selection.  The cost-only launch takes
+// the cost-only twin of the kernel the gradient launch would take (the big kernel where that is the team kernel) and ignores the
+// gradient outputs; it covers discrete rows from caller-provided positions, without the fused dynamics.
+static int rollout_launch(const cb200_rollout_cfg *cfg, const cb200_rollout_io *io, cb200_stream_t stream, bool grad) {
   CB200_DEVICE_GUARD((io != nullptr ? io->cost : nullptr));
-  if (cfg == nullptr || io == nullptr || io->robot_blob == nullptr || io->cost == nullptr || io->grad_q == nullptr ||
+  if (cfg == nullptr || io == nullptr || io->robot_blob == nullptr || io->cost == nullptr || (grad && io->grad_q == nullptr) ||
       io->batch_size < 0 || io->horizon < 1)
+    return ret(cudaErrorInvalidValue);
+  if (!grad && (io->q == nullptr || io->spline != nullptr || io->dynamics != nullptr || cfg->use_sweep != 0))
     return ret(cudaErrorInvalidValue);
   const cb200_spline_input *sp = io->spline;
   if (sp == nullptr && io->q == nullptr) return ret(cudaErrorInvalidValue);
@@ -2497,14 +2587,16 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
   a.pose_tol_t = io->pose_tol_terminal;
   a.pose_tol_nt = io->pose_tol_non_terminal;
   a.cost = io->cost;
-  a.grad_q = io->grad_q;
   a.self_cost = io->self_cost;
   a.scene_cost = io->scene_cost;
   a.pose_cost = io->pose_cost;
   a.cspace_cost = io->cspace_cost;
-  a.grad_vel = io->grad_vel;
-  a.grad_acc = io->grad_acc;
-  a.grad_jerk = io->grad_jerk;
+  if (grad) {
+    a.grad_q = io->grad_q;
+    a.grad_vel = io->grad_vel;
+    a.grad_acc = io->grad_acc;
+    a.grad_jerk = io->grad_jerk;
+  }
   a.link_pos = io->link_pos;
   a.link_quat = io->link_quat;
   a.robot_spheres = io->robot_spheres;
@@ -2525,6 +2617,9 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
   }
   a.blob_smem_bytes = h.smem_bytes;
   a.eval_floats = eval_smem_floats(h.nl, h.D, h.S, h.L, h.n_cl);
+  // row state of the cost-only kernels; the kernel selection below still reads the gradient layout's size
+  const int cost_floats = cost_smem_floats(h.nl, h.D, h.S, h.n_cl, h.n_lp == 0);
+  const int variant_bit = grad ? 0 : CB200_VARIANT_COST_ONLY;
   const bool expand = sp != nullptr && sp->out_position != nullptr && sp->out_velocity != nullptr &&
                       sp->out_acceleration != nullptr && sp->out_jerk != nullptr && sp->out_dt != nullptr;
   // mesh obstacles: scene bit 2.  The in-kernel spline schedule and the fused-dynamics kernel have no mesh build; they refuse mesh
@@ -2598,17 +2693,23 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
     static KernelT const big_arm[4] = {rollout_fused_big_kernel<0, true>, rollout_fused_big_kernel<1, true>,
                                        rollout_fused_big_kernel<2, true>, rollout_fused_big_kernel<3, true>};
     // (an 18-warp build -- 576 threads, 96 registers, small spills -- measured 0.237 ms on G1-29 against 0.219 ms for 16 warps)
-    KernelT bk = arm_sized ? (mesh ? rollout_fused_big_kernel<7, true> : big_arm[scene])
-                           : (mesh ? rollout_fused_big_kernel<7> : big[scene]);
-    const int big_floats = big_smem_floats(h.nl, h.D, h.S, h.L, h.n_cl);
+    static KernelT const cost_big[4] = {rollout_cost_big_kernel<0>, rollout_cost_big_kernel<1>, rollout_cost_big_kernel<2>,
+                                        rollout_cost_big_kernel<3>};
+    static KernelT const cost_big_arm[4] = {rollout_cost_big_kernel<0, true>, rollout_cost_big_kernel<1, true>,
+                                            rollout_cost_big_kernel<2, true>, rollout_cost_big_kernel<3, true>};
+    KernelT bk = grad ? (arm_sized ? (mesh ? rollout_fused_big_kernel<7, true> : big_arm[scene])
+                                   : (mesh ? rollout_fused_big_kernel<7> : big[scene]))
+                      : (arm_sized ? (mesh ? rollout_cost_big_kernel<7, true> : cost_big_arm[scene])
+                                   : (mesh ? rollout_cost_big_kernel<7> : cost_big[scene]));
+    const int big_floats = grad ? big_smem_floats(h.nl, h.D, h.S, h.L, h.n_cl) : cost_floats;
     Plan bp;
     cudaError_t e = cached_plan(PlanKey{(const void *)bk, d.ordinal, (size_t)h.smem_bytes, big_floats, 0, 0, 0}, d,
                                 [](const PlanKey &k, size_t limit) { return plan_warps(k, limit, kBigWarps); }, bp);
     if (e != cudaSuccess) return ret(e);
     // Small batches: a team of warps per row (rollout_fused_team_kernel) when the rows would leave at least half of the
     // resident warp slots idle.  CB200_TEAM = 0 / 2 / 4 forces the team size.  The team kernel has no mesh build: mesh scenes
-    // stay on the big kernel.
-    if (!mesh && h.nl <= 64) {
+    // stay on the big kernel, and so do cost-only launches.
+    if (grad && !mesh && h.nl <= 64) {
       const int team_env = env_int("CB200_TEAM", -1);
       const long long slots = (long long)d.sm_count * kBigWarps;
       // Measured rule.  Small robots (row <= 8 KB, here because of the ESDF): two warps per
@@ -2658,7 +2759,7 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
       long long g = (long long)d.sm_count * bp.per_sm;
       const long long need_ctas = (N + bp.nw - 1) / bp.nw;
       if (g > need_ctas) g = need_ctas;
-      g_last_variant = CB200_VARIANT_BIG;
+      g_last_variant = CB200_VARIANT_BIG | variant_bit;
       CB200_LAUNCH(bk, (int)(g < 1 ? 1 : g), bp.nw * 32, bp.smem, (cudaStream_t)stream, a);
       return finish();
     }
@@ -2715,18 +2816,24 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
     static KernelT const arm_rows[4] = {rollout_fused_kernel<0, false, 3>, rollout_fused_kernel<1, false, 3>,
                                         rollout_fused_kernel<2, false, 3>, rollout_fused_kernel<3, false, 3>};
     static KernelT const arm_pairs[2] = {rollout_fused_kernel<0, false, 3, 2>, rollout_fused_kernel<1, false, 3, 2>};
+    static KernelT const cost_arm_rows[4] = {rollout_cost_kernel<0, 3>, rollout_cost_kernel<1, 3>, rollout_cost_kernel<2, 3>,
+                                             rollout_cost_kernel<3, 3>};
+    static KernelT const cost_arm_pairs[2] = {rollout_cost_kernel<0, 3, 2>, rollout_cost_kernel<1, 3, 2>};
     const int pairs_env = env_int("CB200_ARM_PAIRS", -1);
     const bool pairs = h.nl <= 16 && (scene & 2) == 0 &&
                        (pairs_env >= 0 ? pairs_env != 0 : 2LL * N >= 3LL * d.sm_count * 3 * kWarpsPerCta);
-    kern = pairs ? arm_pairs[scene] : arm_rows[scene];
+    kern = grad ? (pairs ? arm_pairs[scene] : arm_rows[scene]) : (pairs ? cost_arm_pairs[scene] : cost_arm_rows[scene]);
     rows_per_warp = pairs ? 2 : 1;
     arm = true;
   } else {
     static KernelT const fused[2][4] = {
         {rollout_fused_kernel<0, false>, rollout_fused_kernel<1, false>, rollout_fused_kernel<2, false>, rollout_fused_kernel<3, false>},
         {rollout_fused_kernel<0, true>, rollout_fused_kernel<1, true>, rollout_fused_kernel<2, true>, rollout_fused_kernel<3, true>}};
-    kern = mesh ? rollout_fused_kernel<7, false> : fused[spline][scene];
+    static KernelT const cost[4] = {rollout_cost_kernel<0>, rollout_cost_kernel<1>, rollout_cost_kernel<2>, rollout_cost_kernel<3>};
+    if (grad) kern = mesh ? rollout_fused_kernel<7, false> : fused[spline][scene];
+    else kern = mesh ? rollout_cost_kernel<7> : cost[scene];
   }
+  if (!grad) a.eval_floats = cost_floats;
   const cudaError_t e =
       cached_plan(PlanKey{(const void *)kern, d.ordinal, (size_t)h.smem_bytes + halo_bytes, rows_per_warp * a.eval_floats,
                           traj ? io->horizon : 0, 0, 0},
@@ -2742,9 +2849,19 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
   if (grid_ll > need_ctas) grid_ll = need_ctas;
   const int grid = (int)(grid_ll < 1 ? 1 : grid_ll);
   if (need_ctas <= grid_ll) a.work_counter = nullptr;  // every row / pair / tile has its own warp / CTA: nothing to hand out
-  g_last_variant = traj ? CB200_VARIANT_TRAJ : (arm ? CB200_VARIANT_ARM : CB200_VARIANT_STANDARD);
+  g_last_variant = (traj ? CB200_VARIANT_TRAJ : (arm ? CB200_VARIANT_ARM : CB200_VARIANT_STANDARD)) | variant_bit;
   CB200_LAUNCH(kern, grid, nw * 32, p.smem, (cudaStream_t)stream, a);
   return finish();
+}
+
+extern "C" {
+
+int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io *io, cb200_stream_t stream) {
+  return rollout_launch(cfg, io, stream, true);
+}
+
+int cb200_rollout_cost(const cb200_rollout_cfg *cfg, const cb200_rollout_io *io, cb200_stream_t stream) {
+  return rollout_launch(cfg, io, stream, false);
 }
 
 }  // extern "C"

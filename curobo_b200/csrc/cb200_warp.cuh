@@ -144,6 +144,30 @@ __device__ __forceinline__ EvalSmem carve_big_smem(float *base, int nl, int D, i
   return e;
 }
 
+// Row state of the cost-only kernels (rollout_cost_kernel, rollout_cost_big_kernel): nothing the gradient alone reads -- no sphere
+// gradients or gradient list, no force / torque accumulators, no c-space or pose gradients.  `ft` is only the 64-byte index
+// scratch of the second-level self-collision cull.  The padded sphere copy stays for robots without a link-pair list (n_lp == 0),
+// whose pair scan reads it; the others rebuild padded radii from the padding table.
+constexpr int kCullScratchFloats = 16;
+__host__ __device__ inline int cost_smem_floats(int nl, int D, int S, int n_cl, bool padded_copy) {
+  int n = nl * 12 + S * (padded_copy ? 8 : 4) + kCullScratchFloats + n_cl * 4;  // float4-aligned part
+  n += D + n_cl;
+  return (n + 3) & ~3;
+}
+__device__ __forceinline__ EvalSmem carve_cost_smem(float *base, int nl, int D, int S, int n_cl, bool padded_copy) {
+  EvalSmem e;
+  e.cumul = base;
+  e.sph = reinterpret_cast<float4 *>(base + nl * 12);
+  e.gsph = padded_copy ? e.sph + S : nullptr;
+  e.ft = base + nl * 12 + S * (padded_copy ? 8 : 4);
+  e.bc = reinterpret_cast<float4 *>(e.ft + kCullScratchFloats);
+  e.qv = reinterpret_cast<float *>(e.bc + n_cl);
+  e.cmask = reinterpret_cast<uint32_t *>(e.qv + D);
+  e.contrib = e.gqv = e.pose_g = nullptr;
+  e.glist = nullptr;
+  return e;
+}
+
 // Lanes of one row.  W = 32: the whole warp.  W = 16 (paired arm build): half h = lane >> 4 of the warp owns a row of its own,
 // and the two halves may diverge, so every collective of a row names the row's lanes only.  In the helpers below `lane` is the
 // lane within the row (0 .. W-1) and ballots come back in row-local bits.  W = 32 spells exactly the full-warp intrinsics.

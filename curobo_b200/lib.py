@@ -117,7 +117,10 @@ _SIGS = {
     "cb200_robot_blob_bytes": ([C.POINTER(RobotSizes)], C.c_int64),
     "cb200_pack_robot_blob": ([c_p, C.c_int64, C.POINTER(RobotSizes)] + [c_p] * 15, C.c_int64),
     "cb200_rollout_cost_grad": ([C.POINTER(RolloutCfg), C.POINTER(RolloutIO), c_p], _I),
+    "cb200_rollout_cost": ([C.POINTER(RolloutCfg), C.POINTER(RolloutIO), c_p], _I),
 }
+
+VARIANT_COST_ONLY = 0x10    # include/curobo_b200.h: CB200_VARIANT_COST_ONLY, or'd into cb200_last_rollout_variant()
 
 EXPORTED_SYMBOLS = tuple(_SIGS.keys())
 

@@ -283,6 +283,36 @@ class RolloutEngine:
     # -- the hot call --------------------------------------------------------------------------
     def evaluate_action(self, q: torch.Tensor, vel=None, acc=None, jerk=None, dt=None,
                         env_query_idx: Optional[torch.Tensor] = None) -> RolloutOutput:
+        io, B, H = self._state_io(q, vel, acc, jerk, dt)
+        out = self._launch(io, B, H, env_query_idx)
+        if self._effort_cost is not None and vel is not None and acc is not None and jerk is not None and dt is not None:
+            c, gp, gv, ga, _, _ = self._effort_cost.evaluate(q, vel, acc, jerk, dt)
+            out.cspace_cost.add_(c)
+            out.cost.add_(c.sum(-1))
+            out.grad_q.add_(gp)
+            out.grad_vel.add_(gv)
+            out.grad_acc.add_(ga)
+        return out
+
+    def evaluate_cost(self, q: torch.Tensor, vel=None, acc=None, jerk=None, dt=None,
+                      env_query_idx: Optional[torch.Tensor] = None, with_terms: bool = True) -> RolloutOutput:
+        """Cost without gradient (what a sampling-based optimizer such as MPPI evaluates): the rows and cost outputs of
+        evaluate_action from the cost-only kernels, which skip the J^T backward and every other piece of work only the
+        gradient reads.  `grad_q` (and grad_vel / grad_acc / grad_jerk) are left untouched.  `with_terms=False` writes `cost`
+        only -- the per-term tensors keep their previous contents; at particle batch sizes the per-sphere scene_cost alone is
+        ~100 MB of writes.  Discrete rows only (cfg.use_sweep raises ValueError), and the dynamics-aware cost of
+        attach_dynamics is not evaluated here (ValueError).  Buffers are allocated once per (B, H), so the call is CUDA-graph
+        capturable."""
+        if self.cfg.use_sweep:
+            raise ValueError("evaluate_cost covers discrete rows only (cfg.use_sweep = False)")
+        if self._effort_cost is not None or self._dyn_params is not None:
+            raise ValueError("evaluate_cost does not evaluate the dynamics-aware cost of attach_dynamics")
+        io, B, H = self._state_io(q, vel, acc, jerk, dt)
+        return self._launch(io, B, H, env_query_idx, grad=False, with_terms=with_terms)
+
+    def _state_io(self, q, vel, acc, jerk, dt):
+        """Checks the row states of evaluate_action / evaluate_cost, (re)allocates the outputs for their (B, H) and returns the
+        RolloutIO holding them, with B and H."""
         if q.ndim != 3 or q.shape[2] != self.robot.num_dof:
             raise ValueError(f"q must be [B, H, {self.robot.num_dof}], got {tuple(q.shape)}")
         B, H, _ = q.shape
@@ -296,15 +326,7 @@ class RolloutEngine:
             if t is not None:
                 check_tensors(dev, torch.float32, **{name: t})
                 setattr(io, name, t.data_ptr())
-        out = self._launch(io, B, H, env_query_idx)
-        if self._effort_cost is not None and vel is not None and acc is not None and jerk is not None and dt is not None:
-            c, gp, gv, ga, _, _ = self._effort_cost.evaluate(q, vel, acc, jerk, dt)
-            out.cspace_cost.add_(c)
-            out.cost.add_(c.sum(-1))
-            out.grad_q.add_(gp)
-            out.grad_vel.add_(gv)
-            out.grad_acc.add_(ga)
-        return out
+        return io, B, H
 
     def evaluate_knots(self, knots: torch.Tensor, start_state, start_state_idx: torch.Tensor, goal_state,
                        goal_state_idx: torch.Tensor, use_implicit_goal_state: torch.Tensor, bspline_degree: int = 4,
@@ -416,7 +438,7 @@ class RolloutEngine:
             use_implicit_goal_state, B, H, D)
         return out
 
-    def _launch(self, io, B: int, H: int, env_query_idx) -> RolloutOutput:
+    def _launch(self, io, B: int, H: int, env_query_idx, grad: bool = True, with_terms: bool = True) -> RolloutOutput:
         dev = self.device
         o = self.out
         io.robot_blob, io.robot_blob_host = self._blob.data_ptr(), self._blob_host.ctypes.data
@@ -459,10 +481,15 @@ class RolloutEngine:
                 io.cspace_target_dof_weight = tdw.data_ptr()
         if self._sphere_cfgs is not None:
             io.sphere_configs, io.num_sphere_configs = self._sphere_cfgs.data_ptr(), int(self._sphere_cfgs.shape[0])
-        io.cost, io.grad_q = o.cost.data_ptr(), o.grad_q.data_ptr()
-        io.self_cost, io.scene_cost = o.self_cost.data_ptr(), o.scene_cost.data_ptr()
-        io.pose_cost, io.cspace_cost = o.pose_cost.data_ptr(), o.cspace_cost.data_ptr()
-        for name in ("grad_vel", "grad_acc", "grad_jerk", "link_pos", "link_quat", "robot_spheres", "pose_goalset_idx"):
+        io.cost = o.cost.data_ptr()
+        if grad:
+            io.grad_q = o.grad_q.data_ptr()
+        outs = ("grad_vel", "grad_acc", "grad_jerk") if grad else ()
+        if with_terms:
+            io.self_cost, io.scene_cost = o.self_cost.data_ptr(), o.scene_cost.data_ptr()
+            io.pose_cost, io.cspace_cost = o.pose_cost.data_ptr(), o.cspace_cost.data_ptr()
+            outs += ("link_pos", "link_quat", "robot_spheres", "pose_goalset_idx")
+        for name in outs:
             t = getattr(o, name)
             if t is not None:
                 setattr(io, name, t.data_ptr())
@@ -478,8 +505,12 @@ class RolloutEngine:
             if io.spline and not io.spline.contents.out_dt:
                 raise ValueError("mesh obstacles are not supported by the in-kernel spline schedule; use "
                                  "evaluate_knots(in_kernel_spline=False), the expanded schedule")
-        err = self._lib.cb200_rollout_cost_grad(C.byref(self._ccfg), C.byref(io), stream_ptr(dev))
-        _lib.check(err, "rollout_cost_grad")
+        if grad:
+            err = self._lib.cb200_rollout_cost_grad(C.byref(self._ccfg), C.byref(io), stream_ptr(dev))
+            _lib.check(err, "rollout_cost_grad")
+        else:
+            err = self._lib.cb200_rollout_cost(C.byref(self._ccfg), C.byref(io), stream_ptr(dev))
+            _lib.check(err, "rollout_cost")
         return o
 
 

@@ -153,7 +153,12 @@ class B200RobotRollout:
     action space "position_clique": act_seq [B, horizon - 4, D] are waypoints; the state [B, horizon, D] and d/d act_seq come
     from the 5-point stencil with start-state and implicit-goal padding in front of / behind the rollout kernel
     (RolloutEngine.evaluate_positions; the reference's POSITION control space without teleport,
-    transition/fns_state_transition.py:159-308).  Like "bspline" it needs update_params(start_state=..., goal_state=...)."""
+    transition/fns_state_transition.py:159-308).  Like "bspline" it needs update_params(start_state=..., goal_state=...).
+
+    When a call cannot be differentiated -- grad mode off, or `act_seq` does not require grad, as in a particle optimizer or
+    compute_metrics_from_action -- evaluate_action launches the cost-only kernels (RolloutEngine.evaluate_cost) where they
+    cover the rollout (position action space, discrete collision, no dynamics-aware cost attached).  The returned term tensors
+    are the same buffers with the same shapes; `engine.out.grad_q` is not refreshed by such calls."""
 
     def __init__(self, robot: RobotModel, cfg: RolloutConfig, device="cuda:0", cuboid=None, voxel=None, horizon: int = 1,
                  dt: float = 0.05, action_space: str = "position", n_knots: int = 0, bspline_degree: int = 4,
@@ -227,7 +232,14 @@ class B200RobotRollout:
         return self._batch_size
 
     # -- core ----------------------------------------------------------------------------------------------------
-    def _launch(self, act_seq: torch.Tensor):
+    def _cost_only_covers(self) -> bool:
+        """Whether RolloutEngine.evaluate_cost evaluates this rollout's rows: position action space, discrete collision, no
+        dynamics-aware cost attached."""
+        e = self.engine
+        return not (self.is_bspline or self.is_clique or self.cfg.use_sweep or e._effort_cost is not None or
+                    e._dyn_params is not None)
+
+    def _launch(self, act_seq: torch.Tensor, grad: bool = True):
         B = act_seq.shape[0]
         if B != self._batch_size:
             self.update_batch_size(B)
@@ -244,17 +256,24 @@ class B200RobotRollout:
                 raise ValueError("position_clique action space: call update_params(start_state=..., goal_state=...) first")
             return self.engine.evaluate_positions(act_seq, s["start"], s["start_idx"], s["goal"], s["goal_idx"], s["implicit"],
                                                   env_query_idx=self._env_query_idx)
+        evaluate = self.engine.evaluate_action if grad else self.engine.evaluate_cost
         st = self._state
         if st is not None:
-            return self.engine.evaluate_action(act_seq, vel=st.velocity, acc=st.acceleration, jerk=st.jerk, dt=st.dt,
-                                               env_query_idx=self._env_query_idx)
+            return evaluate(act_seq, vel=st.velocity, acc=st.acceleration, jerk=st.jerk, dt=st.dt,
+                            env_query_idx=self._env_query_idx)
         dt = self._dt_tensor if (self.cfg.cspace_type == "state" or self.cfg.use_speed_metric) else None
-        return self.engine.evaluate_action(act_seq, dt=dt, env_query_idx=self._env_query_idx)
+        return evaluate(act_seq, dt=dt, env_query_idx=self._env_query_idx)
 
     def _terms(self, act_seq: torch.Tensor) -> CostsAndConstraints:
         if act_seq.ndim != 3 or act_seq.shape[1] != self._action_horizon or act_seq.shape[2] != self.action_dim:
             raise ValueError(f"act_seq must be [B, {self._action_horizon}, {self.action_dim}], got {tuple(act_seq.shape)}")
-        self_c, scene_c, pose_c, cs_c = FusedTermsFunction.apply(act_seq, self)
+        if self._cost_only_covers() and not (torch.is_grad_enabled() and act_seq.requires_grad):
+            # no gradient can be asked for: the cost-only kernels (engine.out.grad_q is not refreshed)
+            out = self._launch(act_seq, grad=False)
+            self_c, scene_c, pose_c, cs_c = (out.self_cost.detach().unsqueeze(-1), out.scene_cost.detach(), out.pose_cost.detach(),
+                                             out.cspace_cost.detach())
+        else:
+            self_c, scene_c, pose_c, cs_c = FusedTermsFunction.apply(act_seq, self)
         cc = CostsAndConstraints()
         if self.cfg.pose_weight is not None:
             cc.costs.add(pose_c, "tool_pose")

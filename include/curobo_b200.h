@@ -34,8 +34,9 @@ int cb200_abi_version(void);
 int cb200_sm_arch(void);
 /* Human-readable string for the last non-zero return code of this thread (cudaGetErrorString). */
 const char *cb200_error_string(int err);
-/* Which kernel the last cb200_rollout_cost_grad call of this thread launched (introspection for tests and the bench line; the
-   choice is made by the launcher from the robot, the scene content and the row count -- see DESIGN.md "Row scheduling"). */
+/* Which kernel the last cb200_rollout_cost_grad / cb200_rollout_cost call of this thread launched (introspection for tests and the
+   bench line; the choice is made by the launcher from the robot, the scene content and the row count -- see DESIGN.md "Row
+   scheduling").  A cost-only launch reports the variant it twins with CB200_VARIANT_COST_ONLY set. */
 #define CB200_VARIANT_NONE 0
 #define CB200_VARIANT_STANDARD 1 /* rollout_fused_kernel: one warp per row */
 #define CB200_VARIANT_ARM 2      /* ... its 80-register build for arms (one row per warp, or two: one per half-warp) */
@@ -44,6 +45,7 @@ const char *cb200_error_string(int err);
 #define CB200_VARIANT_TEAM4 6    /* ... four warps per row */
 #define CB200_VARIANT_TRAJ 7     /* rollout_traj_kernel: trajectory mode (swept collision, state costs) */
 #define CB200_VARIANT_TRAJ_DYN 8 /* rollout_traj_dyn_kernel: trajectory mode + inverse dynamics */
+#define CB200_VARIANT_COST_ONLY 0x10 /* bit: cb200_rollout_cost (rollout_cost_kernel / rollout_cost_big_kernel) */
 int cb200_last_rollout_variant(void);
 
 /* -------------------------------------------------------------------------------------------
@@ -358,6 +360,13 @@ typedef struct {
 
 int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io *io,
                             cb200_stream_t stream);
+
+/* Cost without gradient: the rows and every cost output of cb200_rollout_cost_grad (cost required; the term costs and the FK
+ * outputs optional), from kernels that skip the J^T backward and everything else only the gradient reads -- what a
+ * sampling-based optimizer (MPPI) evaluates.  grad_q, grad_vel, grad_acc and grad_jerk are ignored and may be NULL.
+ * Covers discrete rows from io->q: use_sweep, a spline front end or dynamics return cudaErrorInvalidValue, as do a NULL
+ * cost, robot_blob or q.  cb200_last_rollout_variant() reports the variant of the kernel it twins | CB200_VARIANT_COST_ONLY. */
+int cb200_rollout_cost(const cb200_rollout_cfg *cfg, const cb200_rollout_io *io, cb200_stream_t stream);
 
 /* -------------------------------------------------------------------------------------------
  * (8f-1) B-spline knot -> state kernels and their adjoint: the step in front of / behind the rollout
