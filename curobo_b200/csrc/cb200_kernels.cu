@@ -1,9 +1,9 @@
 // cb200_kernels.cu -- sm_90a kernels + the C ABI of include/curobo_b200.h.
 //
 // Kernels (all fp32 SIMT; there is no dense contraction on this path, so no tensor cores):
-//   rollout_fused_kernel        persistent, one warp per (seed x waypoint) eval, robot constants staged
-//                               to shared memory with one cp.async.bulk (TMA) per CTA; FK -> spheres ->
-//                               self/scene/pose/c-space cost -> J^T gradient in ONE launch.
+//   rollout_fused_kernel, rollout_fused_big_kernel, rollout_fused_team_kernel, rollout_traj_kernel, rollout_traj_dyn_kernel and
+//   the cost-only rollout_cost_kernel, rollout_cost_big_kernel (select_rollout picks one): persistent CTAs, robot constants staged
+//   by one cp.async.bulk (TMA) per CTA; FK -> spheres -> self/scene/pose/c-space cost -> J^T gradient in ONE launch
 //   kin_forward_kernel          drop-in for kinematics_forward_spheres_kernel
 //   kin_backward_kernel         drop-in for kinematics_backward_kernel
 //   self_collision_kernel       drop-in for self_collision_max_* kernels (single launch)
@@ -16,6 +16,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/curobo_b200.h"
@@ -1766,9 +1767,7 @@ __global__ void __launch_bounds__(128) cspace_position_kernel(const __grid_const
 // ------------------------------------------------------------------------------------------------
 // host helpers
 // ------------------------------------------------------------------------------------------------
-thread_local int g_last_err = 0;
 inline int ret(cudaError_t e) {
-  g_last_err = (int)e;
   if (e != cudaSuccess) (void)cudaGetLastError();  // do not leave a stale error for the caller's next CUDA call
   return (int)e;
 }
@@ -1963,11 +1962,6 @@ __global__ void voxel_mip_kernel(VoxelSet vs, uint16_t *mip, int n_layers) {
     }
     mip[(size_t)k * per + c] = outv;
   }
-}
-
-template <typename T>
-inline void align16(std::vector<unsigned char> &buf) {
-  while (buf.size() % 16) buf.push_back(0);
 }
 
 }  // namespace
@@ -2534,11 +2528,156 @@ int64_t cb200_pack_robot_blob(void *out, int64_t out_bytes, const cb200_robot_si
 
 }  // extern "C"
 
-// cb200_rollout_cost_grad (grad) and cb200_rollout_cost (!grad): one launcher, one kernel selection.  The cost-only launch takes
-// the cost-only twin of the kernel the gradient launch would take (the big kernel where that is the team kernel) and ignores the
-// gradient outputs; it covers discrete rows from caller-provided positions, without the fused dynamics.
-static int rollout_launch(const cb200_rollout_cfg *cfg, const cb200_rollout_io *io, cb200_stream_t stream, bool grad) {
-  CB200_DEVICE_GUARD((io != nullptr ? io->cost : nullptr));
+// One call of the fused rollout launcher as the kernel selection, the kernel table and the launch see it (prepare_rollout).
+struct RolloutShape {
+  BlobHeader h;
+  long long N;                         // rows: batch x H
+  int H, scene;                        // waypoints per trajectory; obstacle types present: bit 0 cuboids, bit 1 voxel grids
+  bool mesh, traj, spline, arm_sized;  // meshes present; trajectory mode; rows from knots in the kernel; arm builds apply
+  bool dynamics, dynamics_ok;          // inverse dynamics asked for (io->dynamics); with what the kernel needs (a.dyn set)
+  int grad_floats, cost_floats;        // shared floats of a row: gradient kernels' standard layout, cost-only kernels
+};
+
+// Rollout kernel families, in the order of their CB200_VARIANT_*; arm rows and arm pairs both report the arm build.
+enum class Family { Standard, ArmRows, ArmPairs, Big, Team2, Team4, Traj, TrajDyn };
+constexpr int kFamilyVariant[] = {CB200_VARIANT_STANDARD, CB200_VARIANT_ARM,   CB200_VARIANT_ARM,  CB200_VARIANT_BIG,
+                                  CB200_VARIANT_TEAM2,    CB200_VARIANT_TEAM4, CB200_VARIANT_TRAJ, CB200_VARIANT_TRAJ_DYN};
+
+// k(std::integral_constant<int, SCENE>) for SCENE = scene: 0..3, or 7 where the family has a mesh build (MESH); else nullptr.
+template <bool MESH, typename K>
+static const void *by_scene(int scene, K k) {
+  using std::integral_constant;
+  if constexpr (MESH) if (scene == 7) return (const void *)k(integral_constant<int, 7>{});
+  const void *const builds[4] = {(const void *)k(integral_constant<int, 0>{}), (const void *)k(integral_constant<int, 1>{}),
+                                 (const void *)k(integral_constant<int, 2>{}), (const void *)k(integral_constant<int, 3>{})};
+  return scene >= 0 && scene < 4 ? builds[scene] : nullptr;
+}
+
+// The kernel of family f for this call, and the one place that names a rollout kernel instantiation.  Kernels are specialised on
+// the obstacle types present so that e.g. the IK kernel carries no ESDF code: the fused kernel's instruction footprint is what
+// limits it.  Mesh scenes take one build per family, SCENE = 7, which checks at run time whether cuboids and ESDF grids are
+// present; the team, arm, fused-dynamics and in-kernel spline builds have none.  nullptr: no such build.
+static const void *rollout_kernel(Family f, bool grad, const RolloutShape &r) {
+  const int s = r.mesh ? 7 : r.scene;
+  switch (f) {
+    case Family::Standard:
+      if (r.spline) return grad ? by_scene<false>(s, [](auto c) { return rollout_fused_kernel<c, true>; }) : nullptr;
+      return by_scene<true>(s, [=](auto c) { return grad ? rollout_fused_kernel<c, false> : rollout_cost_kernel<c>; });
+    case Family::ArmRows:
+      return by_scene<false>(s, [=](auto c) { return grad ? rollout_fused_kernel<c, false, 3> : rollout_cost_kernel<c, 3>; });
+    case Family::ArmPairs:  // never against an ESDF: SCENE 0 and 1 only
+      if (s > 1) return nullptr;
+      if (!grad) return (const void *)(s ? rollout_cost_kernel<1, 3, 2> : rollout_cost_kernel<0, 3, 2>);
+      return (const void *)(s ? rollout_fused_kernel<1, false, 3, 2> : rollout_fused_kernel<0, false, 3, 2>);
+    case Family::Big:
+      if (r.arm_sized)
+        return by_scene<true>(s, [=](auto c) { return grad ? rollout_fused_big_kernel<c, true> : rollout_cost_big_kernel<c, true>; });
+      return by_scene<true>(s, [=](auto c) { return grad ? rollout_fused_big_kernel<c> : rollout_cost_big_kernel<c>; });
+    case Family::Team2: return grad ? by_scene<false>(s, [](auto c) { return rollout_fused_team_kernel<c, 2>; }) : nullptr;
+    case Family::Team4: return grad ? by_scene<false>(s, [](auto c) { return rollout_fused_team_kernel<c, 4>; }) : nullptr;
+    case Family::Traj:
+      if (!grad) return nullptr;
+      if (r.spline && r.arm_sized) return by_scene<false>(s, [](auto c) { return rollout_traj_kernel<c, true, true>; });
+      if (r.spline) return by_scene<false>(s, [](auto c) { return rollout_traj_kernel<c, true>; });
+      if (r.arm_sized) return by_scene<true>(s, [](auto c) { return rollout_traj_kernel<c, false, true>; });
+      return by_scene<true>(s, [](auto c) { return rollout_traj_kernel<c, false>; });
+    case Family::TrajDyn: return grad ? by_scene<false>(s, [](auto c) { return rollout_traj_dyn_kernel<c>; }) : nullptr;
+  }
+  return nullptr;
+}
+
+// Family f planned for this call: its kernel, the shared floats of one of its rows (a.eval_floats) and its CTA shape.
+struct RolloutPlan { Family family; const void *kernel; int row_floats; Plan plan; };
+
+// The kernel family of this call, planned.  The rule reads top to bottom, and a family whose plan does not fit falls to the next
+// candidate: team -> big -> the fused-dynamics, trajectory, arm or standard kernel.  The cost-only launch (!grad) follows the
+// gradient launch's rule, row size included, except that it takes the big kernel where the gradient launch takes the team kernel.
+static cudaError_t select_rollout(const RolloutShape &r, bool grad, const DevInfo &d, RolloutPlan &out) {
+  const BlobHeader &h = r.h;
+  auto plan = [&](Family f, RolloutPlan &p) {
+    const bool team = f == Family::Team2 || f == Family::Team4, dyn = f == Family::TrajDyn;
+    const int team_size = f == Family::Team4 ? 4 : 2;
+    const int big_floats = grad ? big_smem_floats(h.nl, h.D, h.S, h.L, h.n_cl) : r.cost_floats;
+    p.family = f;
+    p.kernel = rollout_kernel(f, grad, r);
+    p.row_floats = team ? (big_floats + team_extra_floats(team_size, h.nl) + 3) & ~3
+                        : f == Family::Big ? big_floats : grad ? r.grad_floats : r.cost_floats;
+    const size_t halo_bytes = r.traj ? (size_t)2 * h.S * sizeof(float4) : 0;  // trajectory kernels: the neighbouring waypoints
+    const PlanKey key{p.kernel, d.ordinal, (size_t)h.smem_bytes + halo_bytes, (f == Family::ArmPairs ? 2 : 1) * p.row_floats,
+                      r.traj ? r.H : 0, dyn ? h.nl : 0, dyn ? h.D : 0};
+    return cached_plan(key, d, [=](const PlanKey &k, size_t limit) {
+      if (dyn) return plan_dyn(k, limit);
+      return team ? plan_team(k, limit, team_size) : plan_warps(k, limit, f == Family::Big ? kBigWarps : kWarpsPerCta);
+    }, p.plan);
+  };
+  // big robots (humanoids) and ESDF scenes, discrete mode: the list-based kernel with up to 16 warps per SM (see
+  // rollout_fused_big_kernel).  CB200_BIG = 0 / 1 forces it off / on.  Default: on when a row of the standard layout exceeds
+  // 8 KB, and against an ESDF for robots that have no 80-register arm build (or too few rows to fill it).
+  // (arms against an ESDF: the 80-register arm build of the standard kernel is faster at full batches -- Franka + 256^3 ESDF,
+  //  16,384 rows: 0.0793 vs 0.0864 ms -- so they come here only when rows are scarce enough for two warps per row)
+  // (an 18-warp build -- 576 threads, 96 registers, small spills -- measured 0.237 ms on G1-29 against 0.219 ms for 16 warps)
+  const int big_env = env_int("CB200_BIG", -1);
+  const long long slots = (long long)d.sm_count * kBigWarps;
+  const bool big_fit = !r.traj && !r.spline && h.n_lp > 0 && h.P > 0;
+  const bool big_want = big_env >= 0 ? big_env != 0
+                                     : ((size_t)r.grad_floats * sizeof(float) > 8192 ||
+                                        ((r.scene & 2) != 0 && (!r.arm_sized || r.N * 2 <= slots)));
+  if (big_fit && big_want) {
+    RolloutPlan big;
+    cudaError_t e = plan(Family::Big, big);
+    if (e != cudaSuccess) return e;
+    // Small batches: a team of warps per row (rollout_fused_team_kernel) when the rows would leave at least half of the
+    // resident warp slots idle.  CB200_TEAM = 0 / 2 / 4 forces the team size.  The team kernel has no mesh build: mesh scenes
+    // stay on the big kernel, and so do cost-only launches.
+    if (grad && !r.mesh && h.nl <= 64) {
+      const int team_env = env_int("CB200_TEAM", -1);
+      // Measured rule.  Small robots (row <= 8 KB, here because of the ESDF): two warps per
+      // row while that leaves warp slots free.  Humanoids: four warps per row while that leaves slots free, then two -- always
+      // when the one-warp plan is shared-memory limited (G1-43: 11 rows per SM; 8 teams of 2 warps are 16 warps
+      // at 8,192 rows), otherwise (G1-29) up to about two rows per warp slot.
+      const bool small_robot = (size_t)r.grad_floats * sizeof(float) <= 8192;
+      const bool smem_limited = big.plan.nw > 0 && big.plan.nw * big.plan.per_sm < kBigWarps;
+      int team = 0;
+      if (team_env >= 0) team = team_env;
+      else if (small_robot) team = (r.N * 2 <= slots) ? 2 : 0;
+      else if (r.N * 4 <= slots) team = 4;
+      else if (smem_limited || r.N <= 2 * slots) team = 2;
+      if (team == 2 || team == 4) {
+        e = plan(team == 4 ? Family::Team4 : Family::Team2, out);
+        if (e != cudaSuccess || out.plan.nw > 0) return e;
+      }
+    }
+    if (big.plan.nw > 0) {
+      out = big;
+      return cudaSuccess;
+    }
+  }
+  if (r.dynamics && !r.dynamics_ok) return cudaErrorInvalidValue;
+  Family f = r.dynamics ? Family::TrajDyn : r.traj ? Family::Traj : Family::Standard;
+  if (!r.traj && !r.spline && !r.mesh && r.arm_sized) {
+    // arms (few links / spheres): the row state is ~3 KB, so residency is register-bound; their 80-register builds keep 24
+    // instead of 16 warps per SM resident and are ~7 % faster on the IK workload (slower for humanoids, where shared memory
+    // bounds residency anyway).
+    // Rows per warp: 2 for arms of <= 16 links (one link per lane of a half-warp in the sparse J^T) from 1.5 rows per resident
+    // warp slot of the arm build (3 CTAs of kWarpsPerCta warps per SM) up; with fewer rows a warp per row is faster (Franka +
+    // cuboids, H100 SXM at 400 W: 0.0183 vs 0.0255 ms at 1.0 rows per slot, 0.0274 vs 0.0270 ms at 1.5, 0.0324 vs 0.0271 ms at
+    // 2.0).  Not against an ESDF: that build spills (140 B) and measured 2 % slower (franka_16384_esdf).  CB200_ARM_PAIRS = 0 / 1
+    // forces one / two rows per warp.
+    // Mesh scenes of arms stay on the 128-register build, one row per warp: an 80-register mesh build spilled 172 B (DESIGN.md
+    // section 4), so none is built.
+    const int pairs_env = env_int("CB200_ARM_PAIRS", -1);
+    const bool pairs = h.nl <= 16 && (r.scene & 2) == 0 &&
+                       (pairs_env >= 0 ? pairs_env != 0 : 2LL * r.N >= 3LL * d.sm_count * 3 * kWarpsPerCta);
+    f = pairs ? Family::ArmPairs : Family::ArmRows;
+  }
+  const cudaError_t e = plan(f, out);
+  if (e != cudaSuccess) return e;
+  return out.plan.nw > 0 ? cudaSuccess : cudaErrorInvalidConfiguration;
+}
+
+// Checks a call's arguments, fills `a` and `r` and runs the expanded spline schedule; r.N == 0 with status 0: nothing to launch.
+static int prepare_rollout(const cb200_rollout_cfg *cfg, const cb200_rollout_io *io, bool grad, cb200_stream_t stream,
+                           FusedArgs &a, RolloutShape &r) {
   if (cfg == nullptr || io == nullptr || io->robot_blob == nullptr || io->cost == nullptr || (grad && io->grad_q == nullptr) ||
       io->batch_size < 0 || io->horizon < 1)
     return ret(cudaErrorInvalidValue);
@@ -2561,14 +2700,13 @@ static int rollout_launch(const cb200_rollout_cfg *cfg, const cb200_rollout_io *
       return ret(cudaErrorInvalidValue);
   }
   if (io->goal_position != nullptr && (io->goal_quat == nullptr || cfg->num_goalset < 1)) return ret(cudaErrorInvalidValue);
-  const long long N = (long long)io->batch_size * io->horizon;
-  if (N == 0) return ret(cudaSuccess);
+  r.H = io->horizon;
+  r.N = (long long)io->batch_size * io->horizon;
+  if (r.N == 0) return ret(cudaSuccess);
   if (io->robot_blob_host == nullptr) return ret(cudaErrorInvalidValue);
-  BlobHeader cached_hdr;
-  memcpy(&cached_hdr, io->robot_blob_host, sizeof(BlobHeader));
-  if (cached_hdr.magic != kBlobMagic || cached_hdr.total_bytes != io->robot_blob_bytes) return ret(cudaErrorInvalidValue);
-  const BlobHeader &h = cached_hdr;
-  FusedArgs a{};
+  memcpy(&r.h, io->robot_blob_host, sizeof(BlobHeader));
+  if (r.h.magic != kBlobMagic || r.h.total_bytes != io->robot_blob_bytes) return ret(cudaErrorInvalidValue);
+  const BlobHeader &h = r.h;
   a.cfg = *cfg;
   a.q = io->q;
   a.vel = io->vel;
@@ -2616,16 +2754,14 @@ static int rollout_launch(const cb200_rollout_cfg *cfg, const cb200_rollout_io *
     a.n_sphere_cfgs = io->num_sphere_configs;
   }
   a.blob_smem_bytes = h.smem_bytes;
-  a.eval_floats = eval_smem_floats(h.nl, h.D, h.S, h.L, h.n_cl);
-  // row state of the cost-only kernels; the kernel selection below still reads the gradient layout's size
-  const int cost_floats = cost_smem_floats(h.nl, h.D, h.S, h.n_cl, h.n_lp == 0);
-  const int variant_bit = grad ? 0 : CB200_VARIANT_COST_ONLY;
+  r.grad_floats = eval_smem_floats(h.nl, h.D, h.S, h.L, h.n_cl);
+  r.cost_floats = cost_smem_floats(h.nl, h.D, h.S, h.n_cl, h.n_lp == 0);
   const bool expand = sp != nullptr && sp->out_position != nullptr && sp->out_velocity != nullptr &&
                       sp->out_acceleration != nullptr && sp->out_jerk != nullptr && sp->out_dt != nullptr;
   // mesh obstacles: scene bit 2.  The in-kernel spline schedule and the fused-dynamics kernel have no mesh build; they refuse mesh
   // scenes rather than drop the meshes (the expanded schedule and the host-composed dynamics cost support them).
-  const bool mesh = cfg->scene_weight > 0.0f && io->meshes != nullptr && io->meshes->inv_pose != nullptr;
-  if (mesh) {
+  r.mesh = cfg->scene_weight > 0.0f && io->meshes != nullptr && io->meshes->inv_pose != nullptr;
+  if (r.mesh) {
     const cb200_mesh_set *m = io->meshes;
     if (m->nodes == nullptr || m->triangles == nullptr || m->node_offset == nullptr || m->triangle_offset == nullptr ||
         m->dims == nullptr || m->enable == nullptr || m->count == nullptr || (sp != nullptr && !expand) || io->dynamics != nullptr)
@@ -2653,205 +2789,69 @@ static int rollout_launch(const cb200_rollout_cfg *cfg, const cb200_rollout_io *
                               sp->start_idx, sp->goal_idx, sp->use_implicit_goal_state, sp->out_position,
                               sp->out_velocity, sp->out_acceleration, sp->out_jerk, sp->n_knots, sp->degree, spline_steps};
   }
-  DevInfo &d = dev_info();
-  const bool traj = cfg->use_sweep != 0;
-  const bool spline = a.spl.knots != nullptr;  // B-spline front end: rows are evaluated from the knots inside the kernel
-  if (traj && cfg->use_speed_metric && a.dt == nullptr && !spline) return ret(cudaErrorInvalidValue);
-  // the adjoint of the spline front end runs right behind the rollout kernel on the same stream
-  auto finish = [&]() -> int {
-    const int rc = launch_status();
-    if (rc != 0 || sp == nullptr || sp->grad_knots == nullptr) return rc;
-    return ret((cudaError_t)cb200_bspline_backward(sp->grad_knots, io->grad_q, io->grad_vel, io->grad_acc, io->grad_jerk,
-                                                   sp->traj_dt, sp->goal_idx, sp->use_implicit_goal_state, io->batch_size,
-                                                   io->horizon, h.D, sp->n_knots, sp->degree, stream));
-  };
-  // kernels are specialised on the obstacle types present (bit 0 cuboids, bit 1 voxel grids) so that e.g. the
-  // IK kernel carries no ESDF code: the fused kernel's instruction footprint is what limits it.  Mesh scenes take one build per
-  // kernel family, SCENE = 7, which checks at run time whether cuboids and ESDF grids are present.
-  const int scene = (cfg->scene_weight > 0.0f ? ((a.cuboids.inv_pose ? 1 : 0) | (a.voxels.inv_pose ? 2 : 0)) : 0);
-  // arms (few links / spheres): the row state is ~3 KB, so residency is register-bound; their 80-register builds keep 24 instead
-  // of 16 warps per SM resident and are ~7 % faster on the IK workload (slower for humanoids, where shared memory bounds
-  // residency anyway)
-  const bool arm_sized = h.nl <= 24 && h.S <= 128;
+  r.traj = cfg->use_sweep != 0;
+  r.spline = a.spl.knots != nullptr;
+  if (r.traj && cfg->use_speed_metric && a.dt == nullptr && !r.spline) return ret(cudaErrorInvalidValue);
+  r.scene = (cfg->scene_weight > 0.0f ? ((a.cuboids.inv_pose ? 1 : 0) | (a.voxels.inv_pose ? 2 : 0)) : 0);
+  r.arm_sized = h.nl <= 24 && h.S <= 128;
+  // inverse dynamics inside the trajectory kernel: rows must come from caller-provided states (or the expanded spline schedule,
+  // which arrives here with a.spl.knots == nullptr) and the STATE c-space cost must be on, else select_rollout refuses the call
+  const cb200_dynamics_params *dp = io->dynamics;
+  r.dynamics = dp != nullptr;
+  r.dynamics_ok = dp != nullptr && dp->link_masses_com != nullptr && dp->link_inertias != nullptr && dp->gravity != nullptr &&
+                  r.traj && cfg->cspace_type == 2 && !r.spline && a.vel != nullptr && a.acc != nullptr;
+  if (r.dynamics_ok) a.dyn = FusedArgs::Dyn{dp->link_masses_com, dp->link_inertias, dp->gravity};
+  return 0;
+}
+
+// cb200_rollout_cost_grad (grad) and cb200_rollout_cost (!grad): one launcher, one kernel selection.  The cost-only launch takes
+// the cost-only twin of the kernel the gradient launch would take (the big kernel where that is the team kernel) and ignores the
+// gradient outputs; it covers discrete rows from caller-provided positions, without the fused dynamics.
+static int rollout_launch(const cb200_rollout_cfg *cfg, const cb200_rollout_io *io, cb200_stream_t stream, bool grad) {
+  CB200_DEVICE_GUARD((io != nullptr ? io->cost : nullptr));
+  FusedArgs a{};
+  RolloutShape r{};
+  int rc = prepare_rollout(cfg, io, grad, stream, a, r);
+  if (rc != 0 || r.N == 0) return rc;
+  const DevInfo &d = dev_info();
+  RolloutPlan c;
+  if (const cudaError_t e = select_rollout(r, grad, d, c); e != cudaSuccess) return ret(e);
+  const Plan &p = c.plan;
+  long long grid, B = io->batch_size, resident = (long long)d.sm_count * p.per_sm;  // resident: CTAs of one wave
+  int block = p.nw * 32;
+  a.eval_floats = c.row_floats;
   // CB200_QUEUE = 0: static striding even when the caller gives a ticket counter
   int32_t *const counter = env_int("CB200_QUEUE", 1) != 0 ? io->work_counter : nullptr;
-  using KernelT = void (*)(const FusedArgs);
-  Plan p;
-  // big robots (humanoids) and ESDF scenes, discrete mode: the list-based kernel with up to 16 warps per SM (see
-  // rollout_fused_big_kernel).  CB200_BIG = 0 / 1 forces it off / on.  Default: on when a row of the standard layout exceeds
-  // 8 KB, and against an ESDF for robots that have no 80-register arm build (or too few rows to fill it).
-  // (arms against an ESDF: the 80-register arm build of the standard kernel is faster at full batches -- Franka + 256^3 ESDF,
-  //  16,384 rows: 0.0793 vs 0.0864 ms -- so they come here only when rows are scarce enough for two warps per row)
-  const int big_env = env_int("CB200_BIG", -1);
-  const bool big_fit = !traj && !spline && h.n_lp > 0 && h.P > 0;
-  const bool big_want = big_env >= 0 ? big_env != 0
-                                     : ((size_t)a.eval_floats * sizeof(float) > 8192 ||
-                                        ((scene & 2) != 0 && (!arm_sized || N * 2 <= (long long)d.sm_count * kBigWarps)));
-  if (big_fit && big_want) {
-    static KernelT const big[4] = {rollout_fused_big_kernel<0>, rollout_fused_big_kernel<1>, rollout_fused_big_kernel<2>,
-                                   rollout_fused_big_kernel<3>};
-    static KernelT const big_arm[4] = {rollout_fused_big_kernel<0, true>, rollout_fused_big_kernel<1, true>,
-                                       rollout_fused_big_kernel<2, true>, rollout_fused_big_kernel<3, true>};
-    // (an 18-warp build -- 576 threads, 96 registers, small spills -- measured 0.237 ms on G1-29 against 0.219 ms for 16 warps)
-    static KernelT const cost_big[4] = {rollout_cost_big_kernel<0>, rollout_cost_big_kernel<1>, rollout_cost_big_kernel<2>,
-                                        rollout_cost_big_kernel<3>};
-    static KernelT const cost_big_arm[4] = {rollout_cost_big_kernel<0, true>, rollout_cost_big_kernel<1, true>,
-                                            rollout_cost_big_kernel<2, true>, rollout_cost_big_kernel<3, true>};
-    KernelT bk = grad ? (arm_sized ? (mesh ? rollout_fused_big_kernel<7, true> : big_arm[scene])
-                                   : (mesh ? rollout_fused_big_kernel<7> : big[scene]))
-                      : (arm_sized ? (mesh ? rollout_cost_big_kernel<7, true> : cost_big_arm[scene])
-                                   : (mesh ? rollout_cost_big_kernel<7> : cost_big[scene]));
-    const int big_floats = grad ? big_smem_floats(h.nl, h.D, h.S, h.L, h.n_cl) : cost_floats;
-    Plan bp;
-    cudaError_t e = cached_plan(PlanKey{(const void *)bk, d.ordinal, (size_t)h.smem_bytes, big_floats, 0, 0, 0}, d,
-                                [](const PlanKey &k, size_t limit) { return plan_warps(k, limit, kBigWarps); }, bp);
-    if (e != cudaSuccess) return ret(e);
-    // Small batches: a team of warps per row (rollout_fused_team_kernel) when the rows would leave at least half of the
-    // resident warp slots idle.  CB200_TEAM = 0 / 2 / 4 forces the team size.  The team kernel has no mesh build: mesh scenes
-    // stay on the big kernel, and so do cost-only launches.
-    if (grad && !mesh && h.nl <= 64) {
-      const int team_env = env_int("CB200_TEAM", -1);
-      const long long slots = (long long)d.sm_count * kBigWarps;
-      // Measured rule.  Small robots (row <= 8 KB, here because of the ESDF): two warps per
-      // row while that leaves warp slots free.  Humanoids: four warps per row while that leaves slots free, then two -- always
-      // when the one-warp plan is shared-memory limited (G1-43: 11 rows per SM; 8 teams of 2 warps are 16 warps
-      // at 8,192 rows), otherwise (G1-29) up to about two rows per warp slot.
-      const bool small_robot = (size_t)a.eval_floats * sizeof(float) <= 8192;
-      const bool smem_limited = bp.nw > 0 && bp.nw * bp.per_sm < kBigWarps;
-      int team = 0;
-      if (team_env >= 0) team = team_env;
-      else if (small_robot) team = (N * 2 <= slots) ? 2 : 0;
-      else if (N * 4 <= slots) team = 4;
-      else if (smem_limited || N <= 2 * slots) team = 2;
-      if (team == 2 || team == 4) {
-        static KernelT const team2[4] = {rollout_fused_team_kernel<0, 2>, rollout_fused_team_kernel<1, 2>,
-                                         rollout_fused_team_kernel<2, 2>, rollout_fused_team_kernel<3, 2>};
-        static KernelT const team4[4] = {rollout_fused_team_kernel<0, 4>, rollout_fused_team_kernel<1, 4>,
-                                         rollout_fused_team_kernel<2, 4>, rollout_fused_team_kernel<3, 4>};
-        KernelT tk = team == 4 ? team4[scene] : team2[scene];
-        const int team_floats = (big_floats + team_extra_floats(team, h.nl) + 3) & ~3;
-        e = cached_plan(PlanKey{(const void *)tk, d.ordinal, (size_t)h.smem_bytes, team_floats, 0, 0, 0}, d,
-                        [team](const PlanKey &k, size_t limit) { return plan_team(k, limit, team); }, p);
-        if (e != cudaSuccess) return ret(e);
-        if (p.nw > 0) {
-          a.eval_floats = team_floats;
-          a.work_counter = counter;
-          const int nteams = p.nw / team;
-          long long g = d.sm_count;
-          const long long need_ctas = (N + nteams - 1) / nteams;
-          // spread the rows over all SMs first: fewer teams per CTA rather than fewer CTAs
-          int launch_teams = nteams;
-          if (need_ctas < g) {
-            launch_teams = (int)((N + g - 1) / g);
-            if (launch_teams < 1) launch_teams = 1;
-          }
-          long long ctas = (N + launch_teams - 1) / launch_teams;
-          if (ctas > g) ctas = g;
-          g_last_variant = team == 4 ? CB200_VARIANT_TEAM4 : CB200_VARIANT_TEAM2;
-          CB200_LAUNCH(tk, (int)(ctas < 1 ? 1 : ctas), launch_teams * team * 32, p.smem, (cudaStream_t)stream, a);
-          return finish();
-        }
-      }
-    }
-    if (bp.nw > 0) {  // (no plan: the standard kernel below)
-      a.eval_floats = big_floats;
-      a.work_counter = counter;
-      long long g = (long long)d.sm_count * bp.per_sm;
-      const long long need_ctas = (N + bp.nw - 1) / bp.nw;
-      if (g > need_ctas) g = need_ctas;
-      g_last_variant = CB200_VARIANT_BIG | variant_bit;
-      CB200_LAUNCH(bk, (int)(g < 1 ? 1 : g), bp.nw * 32, bp.smem, (cudaStream_t)stream, a);
-      return finish();
-    }
+  if (c.family == Family::Team2 || c.family == Family::Team4) {  // at most one CTA per SM
+    const int team = c.family == Family::Team4 ? 4 : 2, nteams = p.nw / team;
+    // spread the rows over all SMs first: fewer teams per CTA rather than fewer CTAs
+    const int launch_teams = (r.N + nteams - 1) / nteams < d.sm_count ? (int)((r.N + d.sm_count - 1) / d.sm_count) : nteams;
+    grid = std::min((r.N + launch_teams - 1) / launch_teams, (long long)d.sm_count);
+    block = launch_teams * team * 32;
+    a.work_counter = counter;
+  } else if (c.family == Family::TrajDyn) {  // a CTA per dynamics chunk of R waypoints, no counter
+    grid = std::min(resident, B * ((r.H + p.R - 1) / p.R));
+  } else {  // a warp per row (standard, arm, big), per pair of rows (paired arm build) or per waypoint of a trajectory tile
+    const int rows = c.family == Family::ArmPairs ? 2 : 1;
+    const long long units = (r.N + rows - 1) / rows;
+    const long long need = r.traj ? B * ((r.H + p.nw - 1) / p.nw) : (units + p.nw - 1) / p.nw;
+    grid = std::min(resident, need);
+    // big: always a counter; the others: none when each row / pair / tile has its own warp / CTA, or when int tickets overflow
+    if (c.family == Family::Big || (need > resident && !(r.traj && need > 0x3fffffffLL))) a.work_counter = counter;
   }
-  const size_t halo_bytes = traj ? (size_t)2 * h.S * sizeof(float4) : 0;
-  if (io->dynamics != nullptr) {
-    // inverse dynamics inside the trajectory kernel: rows must come from caller-provided states (or the expanded spline
-    // schedule, which arrives here with a.spl.knots == nullptr) and the STATE c-space cost must be on
-    const cb200_dynamics_params *dp = io->dynamics;
-    if (dp->link_masses_com == nullptr || dp->link_inertias == nullptr || dp->gravity == nullptr || !traj ||
-        cfg->cspace_type != 2 || spline || a.vel == nullptr || a.acc == nullptr)
-      return ret(cudaErrorInvalidValue);
-    a.dyn = FusedArgs::Dyn{dp->link_masses_com, dp->link_inertias, dp->gravity};
-    using DynKernelT = void (*)(const FusedArgs, const int);
-    static DynKernelT const traj_dyn[4] = {rollout_traj_dyn_kernel<0>, rollout_traj_dyn_kernel<1>, rollout_traj_dyn_kernel<2>,
-                                           rollout_traj_dyn_kernel<3>};
-    DynKernelT dk = traj_dyn[scene];
-    const cudaError_t e = cached_plan(PlanKey{(const void *)dk, d.ordinal, (size_t)h.smem_bytes + halo_bytes, a.eval_floats,
-                                              io->horizon, h.nl, h.D},
-                                      d, plan_dyn, p);
-    if (e != cudaSuccess) return ret(e);
-    if (p.nw == 0) return ret(cudaErrorInvalidConfiguration);
-    long long grid_ll = (long long)d.sm_count * p.per_sm;
-    const long long need_ctas = (long long)io->batch_size * ((io->horizon + p.R - 1) / p.R);
-    if (grid_ll > need_ctas) grid_ll = need_ctas;
-    g_last_variant = CB200_VARIANT_TRAJ_DYN;
-    CB200_LAUNCH(dk, (int)(grid_ll < 1 ? 1 : grid_ll), p.nw * 32, p.smem, (cudaStream_t)stream, a, p.R);
-    return finish();
-  }
-  // standard, arm and trajectory kernels: one warp per row (per pair of rows in the arms' paired build, per waypoint of a
-  // trajectory tile)
-  KernelT kern;
-  int rows_per_warp = 1;
-  bool arm = false;
-  if (traj) {
-    static KernelT const traj_full[2][4] = {
-        {rollout_traj_kernel<0, false>, rollout_traj_kernel<1, false>, rollout_traj_kernel<2, false>, rollout_traj_kernel<3, false>},
-        {rollout_traj_kernel<0, true>, rollout_traj_kernel<1, true>, rollout_traj_kernel<2, true>, rollout_traj_kernel<3, true>}};
-    static KernelT const traj_small[2][4] = {
-        {rollout_traj_kernel<0, false, true>, rollout_traj_kernel<1, false, true>, rollout_traj_kernel<2, false, true>,
-         rollout_traj_kernel<3, false, true>},
-        {rollout_traj_kernel<0, true, true>, rollout_traj_kernel<1, true, true>, rollout_traj_kernel<2, true, true>,
-         rollout_traj_kernel<3, true, true>}};
-    if (arm_sized) kern = mesh ? rollout_traj_kernel<7, false, true> : traj_small[spline][scene];
-    else kern = mesh ? rollout_traj_kernel<7, false> : traj_full[spline][scene];
-  } else if (!spline && !mesh && arm_sized) {
-    // rows per warp: 2 for arms of <= 16 links (one link per lane of a half-warp in the sparse J^T) from 1.5 rows per resident
-    // warp slot of the arm build (3 CTAs of kWarpsPerCta warps per SM) up; with fewer rows a warp per row is faster (Franka +
-    // cuboids, H100 SXM at 400 W: 0.0183 vs 0.0255 ms at 1.0 rows per slot, 0.0274 vs 0.0270 ms at 1.5, 0.0324 vs 0.0271 ms at
-    // 2.0).  Not against an ESDF: that build spills (140 B) and measured 2 % slower (franka_16384_esdf).  CB200_ARM_PAIRS = 0 / 1
-    // forces one / two rows per warp.
-    // Mesh scenes of arms stay on the 128-register build, one row per warp: an 80-register mesh build spilled 172 B (DESIGN.md
-    // section 4), so none is built.
-    static KernelT const arm_rows[4] = {rollout_fused_kernel<0, false, 3>, rollout_fused_kernel<1, false, 3>,
-                                        rollout_fused_kernel<2, false, 3>, rollout_fused_kernel<3, false, 3>};
-    static KernelT const arm_pairs[2] = {rollout_fused_kernel<0, false, 3, 2>, rollout_fused_kernel<1, false, 3, 2>};
-    static KernelT const cost_arm_rows[4] = {rollout_cost_kernel<0, 3>, rollout_cost_kernel<1, 3>, rollout_cost_kernel<2, 3>,
-                                             rollout_cost_kernel<3, 3>};
-    static KernelT const cost_arm_pairs[2] = {rollout_cost_kernel<0, 3, 2>, rollout_cost_kernel<1, 3, 2>};
-    const int pairs_env = env_int("CB200_ARM_PAIRS", -1);
-    const bool pairs = h.nl <= 16 && (scene & 2) == 0 &&
-                       (pairs_env >= 0 ? pairs_env != 0 : 2LL * N >= 3LL * d.sm_count * 3 * kWarpsPerCta);
-    kern = grad ? (pairs ? arm_pairs[scene] : arm_rows[scene]) : (pairs ? cost_arm_pairs[scene] : cost_arm_rows[scene]);
-    rows_per_warp = pairs ? 2 : 1;
-    arm = true;
-  } else {
-    static KernelT const fused[2][4] = {
-        {rollout_fused_kernel<0, false>, rollout_fused_kernel<1, false>, rollout_fused_kernel<2, false>, rollout_fused_kernel<3, false>},
-        {rollout_fused_kernel<0, true>, rollout_fused_kernel<1, true>, rollout_fused_kernel<2, true>, rollout_fused_kernel<3, true>}};
-    static KernelT const cost[4] = {rollout_cost_kernel<0>, rollout_cost_kernel<1>, rollout_cost_kernel<2>, rollout_cost_kernel<3>};
-    if (grad) kern = mesh ? rollout_fused_kernel<7, false> : fused[spline][scene];
-    else kern = mesh ? rollout_cost_kernel<7> : cost[scene];
-  }
-  if (!grad) a.eval_floats = cost_floats;
-  const cudaError_t e =
-      cached_plan(PlanKey{(const void *)kern, d.ordinal, (size_t)h.smem_bytes + halo_bytes, rows_per_warp * a.eval_floats,
-                          traj ? io->horizon : 0, 0, 0},
-                  d, [](const PlanKey &k, size_t limit) { return plan_warps(k, limit, kWarpsPerCta); }, p);
-  if (e != cudaSuccess) return ret(e);
-  if (p.nw == 0) return ret(cudaErrorInvalidConfiguration);
-  const int nw = p.nw;
-  a.work_counter = counter;
-  if (traj && (long long)io->batch_size * ((io->horizon + nw - 1) / nw) > 0x3fffffffLL) a.work_counter = nullptr;  // int tickets
-  long long grid_ll = (long long)d.sm_count * p.per_sm;
-  const long long units = (N + rows_per_warp - 1) / rows_per_warp;  // rows, or pairs of rows
-  const long long need_ctas = traj ? (long long)io->batch_size * ((io->horizon + nw - 1) / nw) : (units + nw - 1) / nw;
-  if (grid_ll > need_ctas) grid_ll = need_ctas;
-  const int grid = (int)(grid_ll < 1 ? 1 : grid_ll);
-  if (need_ctas <= grid_ll) a.work_counter = nullptr;  // every row / pair / tile has its own warp / CTA: nothing to hand out
-  g_last_variant = (traj ? CB200_VARIANT_TRAJ : (arm ? CB200_VARIANT_ARM : CB200_VARIANT_STANDARD)) | variant_bit;
-  CB200_LAUNCH(kern, grid, nw * 32, p.smem, (cudaStream_t)stream, a);
-  return finish();
+  const int g = (int)std::max(grid, 1LL);
+  g_last_variant = kFamilyVariant[(int)c.family] | (grad ? 0 : CB200_VARIANT_COST_ONLY);
+  if (c.family == Family::TrajDyn)
+    CB200_LAUNCH(((void (*)(const FusedArgs, const int))c.kernel), g, block, p.smem, (cudaStream_t)stream, a, p.R);
+  else
+    CB200_LAUNCH(((void (*)(const FusedArgs))c.kernel), g, block, p.smem, (cudaStream_t)stream, a);
+  rc = launch_status();
+  // the adjoint of the spline front end runs right behind the rollout kernel on the same stream
+  const cb200_spline_input *sp = io->spline;
+  if (rc != 0 || sp == nullptr || sp->grad_knots == nullptr) return rc;
+  return ret((cudaError_t)cb200_bspline_backward(sp->grad_knots, io->grad_q, io->grad_vel, io->grad_acc, io->grad_jerk,
+                                                 sp->traj_dt, sp->goal_idx, sp->use_implicit_goal_state, io->batch_size,
+                                                 io->horizon, r.h.D, sp->n_knots, sp->degree, stream));
 }
 
 extern "C" {
