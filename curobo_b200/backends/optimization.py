@@ -125,3 +125,64 @@ def launch_lbfgs_step(
         int(bool(fix_terminal_action)), stream_ptr(dev))
     _lib.check(err, "launch_lbfgs_step")
     return [step_vec, rho_buffer, y_buffer, s_buffer, x_0, grad_0]
+
+
+def launch_mppi_sample(actions: torch.Tensor, mean: torch.Tensor, scale: torch.Tensor, noise: torch.Tensor,
+                       lows: torch.Tensor, highs: torch.Tensor, num_neg: int = 0) -> torch.Tensor:
+    """MPPI particles (ParticleOptCore.sample_actions, DIAG_A + CLAMP) into actions [P, Np, H, D]: per problem the
+    Ns = noise.shape[1] sampled particles mean + noise * scale, then `num_neg` copies of -mean, then zeros, clamped to
+    [lows, highs].  mean [P, H, D], scale [P, D], noise [P or 1, Ns, H, D] (1: one sample set for every problem),
+    lows / highs [D].  This library's extension of the reference's kernel set (the reference builds particles in torch)."""
+    dev = actions.device
+    check_tensors(dev, torch.float32, actions=actions, mean=mean, scale=scale, noise=noise, lows=lows, highs=highs)
+    if actions.ndim != 4:
+        raise ValueError(f"actions must be [P, Np, H, D], got {tuple(actions.shape)}")
+    P, Np, H, D = actions.shape
+    if noise.ndim != 4 or noise.shape[0] not in (1, P) or tuple(noise.shape[2:]) != (H, D):
+        raise ValueError(f"noise must be [{P} or 1, Ns, {H}, {D}], got {tuple(noise.shape)}")
+    Ns = int(noise.shape[1])
+    if tuple(mean.shape) != (P, H, D) or tuple(scale.shape) != (P, D) or lows.numel() != D or highs.numel() != D:
+        raise ValueError("mean must be [P, H, D], scale [P, D], lows / highs [D]")
+    if Ns < 1 or num_neg < 0 or Ns + num_neg > Np:
+        raise ValueError(f"{Ns} sampled + {num_neg} negated particles do not fit {Np} particles")
+    if P == 0:
+        return actions                        # empty tensors have no storage to hand the kernel
+    err = _lib.load().cb200_mppi_sample(actions.data_ptr(), mean.data_ptr(), scale.data_ptr(), noise.data_ptr(), lows.data_ptr(),
+                                        highs.data_ptr(), P, Np, Ns, int(num_neg), H, D, int(noise.shape[0] == P and P > 1),
+                                        stream_ptr(dev))
+    _lib.check(err, "launch_mppi_sample")
+    return actions
+
+
+def launch_mppi_update(actions: torch.Tensor, cost: torch.Tensor, mean: torch.Tensor, cov: Optional[torch.Tensor],
+                       scale: Optional[torch.Tensor], best: Optional[torch.Tensor], beta: float, step_size_mean: float,
+                       step_size_cov: float, kappa: float, discount: float = 1.0) -> None:
+    """MPPI distribution update (MPPI._update_distribution with jit_mean_cov_diag_a) from actions [P, Np, H, D] and their
+    row costs [P * Np, H], in place: mean [P, H, D]; cov / scale [P, D] when both are given (update_cov); best [P, H, D]
+    = the particle of largest weight when given (BEST mode).  `discount` = sum_h gamma^h / gamma^0."""
+    dev = mean.device
+    check_tensors(dev, torch.float32, actions=actions, cost=cost, mean=mean)
+    if actions.ndim != 4:
+        raise ValueError(f"actions must be [P, Np, H, D], got {tuple(actions.shape)}")
+    P, Np, H, D = actions.shape
+    if cost.numel() != P * Np * H or cost.shape[0] != P * Np or tuple(mean.shape) != (P, H, D):
+        raise ValueError(f"cost must be [{P * Np}, {H}] and mean [{P}, {H}, {D}]")
+    if (cov is None) != (scale is None):
+        raise ValueError("cov and scale are updated together: pass both or neither")
+    if cov is not None:
+        check_tensors(dev, torch.float32, cov=cov, scale=scale)
+        if tuple(cov.shape) != (P, D) or tuple(scale.shape) != (P, D):
+            raise ValueError(f"cov / scale must be [{P}, {D}]")
+    if best is not None:
+        check_tensors(dev, torch.float32, best=best)
+        if tuple(best.shape) != (P, H, D):
+            raise ValueError(f"best must be [{P}, {H}, {D}]")
+    if not beta > 0.0:
+        raise ValueError("beta must be positive")
+    if P == 0:
+        return
+    p = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+    err = _lib.load().cb200_mppi_update(actions.data_ptr(), cost.data_ptr(), mean.data_ptr(), p(cov), p(scale), p(best), P, Np, H, D,
+                                        float(beta), float(step_size_mean), float(step_size_cov), float(kappa), float(discount),
+                                        int(cov is not None), int(best is not None), stream_ptr(dev))
+    _lib.check(err, "launch_mppi_update")

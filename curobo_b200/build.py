@@ -165,14 +165,16 @@ def build_reference_legacy_kernels(force: bool = False, verbose: bool = False):
 
 def build_reference_callsites(force: bool = False, verbose: bool = False):
     """oracle/_ref/pyref: the reference's Python call sites of the kernel backends (cuda_ops/*.py and their import closure)
-    compiled to byte code from the sources where they lie (recipe: oracle/build_pyref.py; test infrastructure, git-ignored,
-    travels to the GPU box).  Returns the directory, or None when /root/reference is absent and nothing was built before."""
+    compiled to byte code from the sources where they lie (recipe: oracle/build_pyref.py, run through
+    oracle/build_pyref_particle.py, which adds the reference's MPPI optimizer; test infrastructure, git-ignored, travels to the
+    GPU box).  Returns the directory, or None when /root/reference is absent and nothing was built before."""
     out = os.path.join(ROOT, "oracle", "_ref", "pyref")
     manifest = os.path.join(out, "MANIFEST.json")
-    recipe = os.path.join(ROOT, "oracle", "build_pyref.py")
-    if not os.path.isdir(REFERENCE) or not os.path.exists(recipe):
+    recipes = [os.path.join(ROOT, "oracle", f) for f in ("build_pyref.py", "build_pyref_particle.py")]
+    recipe = recipes[-1]
+    if not os.path.isdir(REFERENCE) or not all(os.path.exists(r) for r in recipes):
         return out if os.path.exists(manifest) else None
-    if not force and _newer(manifest, [recipe]):
+    if not force and _newer(manifest, recipes):
         return out
     _run([sys.executable, recipe], verbose)          # own process: the recipe installs import stubs
     return out

@@ -3,6 +3,8 @@
 //   cb200_lbfgs_step    replaces kernel_lbfgs_step / kernel_lbfgs_step_shared_memory
 //                       (curobo/_src/curobolib/kernels/optimization/lbfgs/lbfgs_step_kernel.cuh:39-199)
 //   cb200_line_search   replaces kernel_line_search (optimization/line_search/line_search_kernel.cuh:60-199)
+//   cb200_mppi_sample   replaces the torch particle construction of ParticleOptCore.sample_actions
+//   cb200_mppi_update   replaces the torch softmax / weighted sums / blends of MPPI._update_distribution (DIAG_A)
 //
 // The reference launches ONE CTA OF v_dim THREADS PER PROBLEM (optimization_config.py:54-70,76-127): 16,384 CTAs of
 // 7 threads for the IK headline.  Here the mapping follows the problem size instead:
@@ -451,6 +453,205 @@ int launch_ls_group(const LineSearchArgs &a, cudaStream_t stream) {
   CB200_LAUNCH(line_search_group_kernel<G>, grid, block, 0, stream, a);
   return status(cudaGetLastError());
 }
+
+// ---- MPPI sample -----------------------------------------------------------------------------------------------------
+// ParticleOptCore.sample_actions (optim/components/particle_opt_core.py:409-441) for DIAG_A covariance and CLAMP squash:
+// per problem, Ns particles mean + noise * scale, then n_neg copies of -mean, then zeros; every element clamped to
+// max(min(a, high), low).  One thread per element of actions [P, Np, H, D], d fastest.  The explicit roundings keep torch's
+// two (mul, then add) under --fmad=true, so the actions equal the reference's bit for bit.
+struct MppiSampleArgs {
+  float *actions;
+  const float *mean, *scale, *noise, *lows, *highs;
+  int total, Np, Ns, n_neg, HD, D, noise_stride;  // noise_stride: floats between problems' sample sets (0: one shared set)
+};
+
+__global__ void __launch_bounds__(256) mppi_sample_kernel(const __grid_constant__ MppiSampleArgs a) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.total) return;
+  const int d = i % a.D, hd = i % a.HD, pj = i / a.HD;
+  const int j = pj % a.Np, p = pj / a.Np;
+  float v = 0.0f;
+  if (j < a.Ns)
+    v = __fadd_rn(a.mean[p * a.HD + hd], __fmul_rn(a.noise[p * a.noise_stride + j * a.HD + hd], a.scale[p * a.D + d]));
+  else if (j < a.Ns + a.n_neg)
+    v = -a.mean[p * a.HD + hd];
+  a.actions[i] = fmaxf(fminf(v, a.highs[d]), a.lows[d]);
+}
+
+// ---- MPPI update -----------------------------------------------------------------------------------------------------
+// MPPI._update_distribution (optim/particle/mppi.py:200-248) with jit_mean_cov_diag_a (mppi.py:722-757), per problem:
+//   total_j = discount * sum_h cost[j, h]          (the reference sums the horizon, then broadcasts gamma_seq over it)
+//   w = softmax(-total / beta)                     (max subtracted)
+//   best = a[argmax_j w_j]                         (lowest index on ties, torch.argmax)
+//   cov_upd[d] = mean_h sum_j w_j (a_j[h,d] - mean_old[h,d])^2,  cov = (1-s_c) cov + s_c cov_upd + kappa,  scale = sqrt(cov)
+//   mean = (1-s_m) mean + s_m sum_j w_j a_j
+// The library builds with --prec-sqrt=false; scale takes the correctly rounded square root torch.sqrt gives (the host SIMT
+// emulation's std::sqrt is correctly rounded too).
+#ifdef CB200_SIMT_EMULATION
+inline float sqrt_rn(float x) { return std::sqrt(x); }
+#else
+__device__ __forceinline__ float sqrt_rn(float x) { return __fsqrt_rn(x); }
+#endif
+// Every sum runs in one fixed order (per-lane serial, then a fixed shuffle tree), so runs and graph replays are bit-identical.
+struct MppiUpdateArgs {
+  const float *actions, *cost;
+  float *mean, *cov, *scale, *best;
+  int P, Np, H, D;
+  float neg_inv_beta, discount, step_mean, keep_mean, step_cov, keep_cov, kappa;
+  int update_cov, best_mode;
+};
+
+// the particle's softmax argument -total / beta
+__device__ __forceinline__ float mppi_exponent(const MppiUpdateArgs &a, long long p, int j) {
+  const float *c = a.cost + ((size_t)p * a.Np + j) * a.H;
+  float s = 0.0f;
+  for (int h = 0; h < a.H; ++h) s = __fadd_rn(s, c[h]);
+  return __fmul_rn(a.neg_inv_beta, __fmul_rn(a.discount, s));
+}
+
+// (weight, index) of the larger weight, the lower index on ties
+__device__ __forceinline__ void argmax_merge(float &w, int &j, float ow, int oj) {
+  if (ow > w || (ow == w && oj < j)) {
+    w = ow;
+    j = oj;
+  }
+}
+
+// mean / best for element v of problem p from the weights w[Np]; returns the element's covariance-update sum
+__device__ __forceinline__ float mppi_element(const MppiUpdateArgs &a, long long p, int v, const float *w, int best_j) {
+  const int V = a.H * a.D;
+  const float *act = a.actions + (size_t)p * a.Np * V + v;
+  const float mo = a.mean[(size_t)p * V + v];
+  float m = 0.0f, c = 0.0f;
+  for (int j = 0; j < a.Np; ++j) {
+    const float x = act[(size_t)j * V], wj = w[j];
+    const float dl = __fsub_rn(x, mo);
+    m = __fadd_rn(m, __fmul_rn(wj, x));
+    c = __fadd_rn(c, __fmul_rn(wj, __fmul_rn(dl, dl)));
+  }
+  a.mean[(size_t)p * V + v] = __fadd_rn(__fmul_rn(a.keep_mean, mo), __fmul_rn(a.step_mean, m));
+  if (a.best_mode) a.best[(size_t)p * V + v] = act[(size_t)best_j * V];
+  return c;
+}
+
+// covariance of dimension d from the per-element sums sv[H*D]
+__device__ __forceinline__ void mppi_cov(const MppiUpdateArgs &a, long long p, int d, const float *sv) {
+  float s = 0.0f;
+  for (int h = 0; h < a.H; ++h) s = __fadd_rn(s, sv[h * a.D + d]);
+  const size_t o = (size_t)p * a.D + d;
+  const float upd = __fdiv_rn(s, (float)a.H);
+  const float cv = __fadd_rn(__fadd_rn(__fmul_rn(a.keep_cov, a.cov[o]), __fmul_rn(a.step_cov, upd)), a.kappa);
+  a.cov[o] = cv;
+  a.scale[o] = sqrt_rn(cv);
+}
+
+// small problems (Np * V <= kMppiGroupElems): a group of G lanes owns a problem, 128 / G problems per CTA, no __syncthreads
+constexpr int kMppiGroupElems = 2048, kMppiGroupSmem = 256;  // group path also needs Np + V <= kMppiGroupSmem
+template <int G>
+__global__ void __launch_bounds__(128) mppi_update_group_kernel(const __grid_constant__ MppiUpdateArgs a) {
+  CB200_EXTERN_SHARED float smem[];
+  const int t = threadIdx.x % G, grp = threadIdx.x / G;
+  const int Np = a.Np, D = a.D, V = a.H * a.D;
+  float *w = smem + (size_t)grp * (Np + V), *sv = w + Np;  // weights, then the covariance-update sums
+  const long long p = (long long)blockIdx.x * (128 / G) + grp;
+  const bool valid = p < a.P;
+  float mx = -INFINITY;
+  for (int j = t; j < Np; j += G) {
+    const float x = valid ? mppi_exponent(a, p, j) : 0.0f;
+    w[j] = x;
+    mx = fmaxf(mx, x);
+  }
+  mx = group_max<G>(mx);
+  float se = 0.0f;
+  for (int j = t; j < Np; j += G) {
+    const float e = expf(__fsub_rn(w[j], mx));
+    w[j] = e;
+    se = __fadd_rn(se, e);
+  }
+  se = group_sum<G>(se);
+  float bw = -1.0f;
+  int bj = 0;
+  for (int j = t; j < Np; j += G) {
+    const float wj = __fdiv_rn(w[j], se);
+    w[j] = wj;
+    argmax_merge(bw, bj, wj, j);
+  }
+#pragma unroll
+  for (int off = G / 2; off > 0; off >>= 1) {
+    const float ow = __shfl_xor_sync(kFull, bw, off, G);
+    const int oj = __shfl_xor_sync(kFull, bj, off, G);
+    argmax_merge(bw, bj, ow, oj);
+  }
+  __syncwarp();  // every lane's weights before any lane reads them all
+  if (valid)
+    for (int v = t; v < V; v += G) sv[v] = mppi_element(a, p, v, w, bj);
+  if (a.update_cov) {
+    __syncwarp();
+    if (valid)
+      for (int d = t; d < D; d += G) mppi_cov(a, p, d, sv);
+  }
+}
+
+// larger problems: one CTA per problem, block reductions through shared memory (Np + V floats, within the default 48 KB)
+constexpr int kMppiBlock = 256, kMppiMaxSmemFloats = 48 * 1024 / 4;
+__global__ void __launch_bounds__(kMppiBlock) mppi_update_block_kernel(const __grid_constant__ MppiUpdateArgs a) {
+  CB200_EXTERN_SHARED float smem[];
+  __shared__ float data[32];
+  __shared__ float arg_w[32];
+  __shared__ int arg_j[32];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5, nt = blockDim.x;
+  const int Np = a.Np, D = a.D, V = a.H * a.D;
+  float *w = smem, *sv = smem + Np;
+  const long long p = blockIdx.x;
+  float mx = -INFINITY;
+  for (int j = t; j < Np; j += nt) {
+    const float x = mppi_exponent(a, p, j);
+    w[j] = x;
+    mx = fmaxf(mx, x);
+  }
+  mx = block_max(mx, data);
+  float se = 0.0f;
+  for (int j = t; j < Np; j += nt) {
+    const float e = expf(__fsub_rn(w[j], mx));
+    w[j] = e;
+    se = __fadd_rn(se, e);
+  }
+  se = block_sum(se, data);
+  float bw = -1.0f;
+  int bj = 0;
+  for (int j = t; j < Np; j += nt) {
+    const float wj = __fdiv_rn(w[j], se);
+    w[j] = wj;
+    argmax_merge(bw, bj, wj, j);
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    const float ow = __shfl_xor_sync(kFull, bw, off);
+    const int oj = __shfl_xor_sync(kFull, bj, off);
+    argmax_merge(bw, bj, ow, oj);
+  }
+  if (lane == 0) {
+    arg_w[warp] = bw;
+    arg_j[warp] = bj;
+  }
+  __syncthreads();  // also orders every thread's weights before the reads below
+  bw = -1.0f;
+  bj = 0;
+  for (int k = 0; k < (nt >> 5); ++k) argmax_merge(bw, bj, arg_w[k], arg_j[k]);
+  for (int v = t; v < V; v += nt) sv[v] = mppi_element(a, p, v, w, bj);
+  if (a.update_cov) {
+    __syncthreads();
+    for (int d = t; d < D; d += nt) mppi_cov(a, p, d, sv);
+  }
+}
+
+template <int G>
+int launch_mppi_group(const MppiUpdateArgs &a, cudaStream_t stream) {
+  constexpr int NG = 128 / G;
+  const size_t smem = (size_t)NG * (a.Np + a.H * a.D) * sizeof(float);
+  CB200_LAUNCH(mppi_update_group_kernel<G>, (a.P + NG - 1) / NG, 128, smem, stream, a);
+  return status(cudaGetLastError());
+}
 }  // namespace
 
 extern "C" {
@@ -512,6 +713,47 @@ int cb200_line_search(float *best_cost, float *best_action, int16_t *best_iterat
   if (opt_dim <= 32) return launch_ls_group<32>(a, st);
   const int block = (opt_dim + 31) / 32 * 32;
   CB200_LAUNCH(line_search_block_kernel, batchsize, block, 0, st, a);
+  return status(cudaGetLastError());
+}
+
+int cb200_mppi_sample(float *actions, const float *mean, const float *scale, const float *noise, const float *lows,
+                      const float *highs, int num_problems, int num_particles, int num_sampled, int num_neg, int horizon,
+                      int action_dim, int noise_per_problem, cb200_stream_t stream) {
+  CB200_DEVICE_GUARD(actions);
+  if (actions == nullptr || mean == nullptr || scale == nullptr || noise == nullptr || lows == nullptr || highs == nullptr ||
+      num_problems < 0 || num_particles < 1 || num_sampled < 1 || num_neg < 0 || num_sampled + num_neg > num_particles ||
+      horizon < 1 || action_dim < 1 ||
+      (long long)num_problems * num_particles * horizon * action_dim > 0x7fffffffLL)
+    return status(cudaErrorInvalidValue);
+  if (num_problems == 0) return status(cudaSuccess);
+  const int HD = horizon * action_dim, total = num_problems * num_particles * HD;
+  MppiSampleArgs a{actions, mean, scale, noise, lows, highs, total, num_particles, num_sampled, num_neg, HD, action_dim,
+                   noise_per_problem ? num_sampled * HD : 0};
+  CB200_LAUNCH(mppi_sample_kernel, (total + 255) / 256, 256, 0, (cudaStream_t)stream, a);
+  return status(cudaGetLastError());
+}
+
+int cb200_mppi_update(const float *actions, const float *cost, float *mean, float *cov, float *scale, float *best,
+                      int num_problems, int num_particles, int horizon, int action_dim, float beta, float step_size_mean,
+                      float step_size_cov, float kappa, float discount, int update_cov, int best_mode, cb200_stream_t stream) {
+  CB200_DEVICE_GUARD(mean);
+  const long long V = (long long)horizon * action_dim;
+  if (actions == nullptr || cost == nullptr || mean == nullptr || (update_cov && (cov == nullptr || scale == nullptr)) ||
+      (best_mode && best == nullptr) || num_problems < 0 || num_particles < 1 || horizon < 1 || action_dim < 1 ||
+      !(beta > 0.0f) || num_particles + V > kMppiMaxSmemFloats)
+    return status(cudaErrorInvalidValue);
+  if (num_problems == 0) return status(cudaSuccess);
+  // the coefficients as torch forms them: Python-double scalars rounded once to float
+  MppiUpdateArgs a{actions, cost, mean, cov, scale, best, num_problems, num_particles, horizon, action_dim,
+                   (float)(-1.0 / (double)beta), discount, step_size_mean, (float)(1.0 - (double)step_size_mean),
+                   step_size_cov, (float)(1.0 - (double)step_size_cov), kappa, update_cov ? 1 : 0, best_mode ? 1 : 0};
+  cudaStream_t st = (cudaStream_t)stream;
+  if ((long long)num_particles * V <= kMppiGroupElems && num_particles + V <= kMppiGroupSmem) {
+    if (V <= 8) return launch_mppi_group<8>(a, st);
+    if (V <= 16) return launch_mppi_group<16>(a, st);
+    return launch_mppi_group<32>(a, st);
+  }
+  CB200_LAUNCH(mppi_update_block_kernel, num_problems, kMppiBlock, (num_particles + V) * sizeof(float), st, a);
   return status(cudaGetLastError());
 }
 

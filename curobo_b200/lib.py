@@ -99,6 +99,8 @@ _SIGS = {
     "cb200_acceleration_integrate": ([c_p] * 10 + [_I] * 4 + [c_p], _I),
     "cb200_lbfgs_step": ([c_p] * 8 + [C.c_float] + [_I] * 4 + [c_p] * 3 + [_I, c_p, _I, _I, c_p], _I),
     "cb200_line_search": ([c_p] * 5 + [_I, C.c_float, C.c_float] + [c_p] * 13 + [C.c_float, C.c_float] + [_I] * 5 + [c_p], _I),
+    "cb200_mppi_sample": ([c_p] * 6 + [_I] * 7 + [c_p], _I),
+    "cb200_mppi_update": ([c_p] * 6 + [_I] * 4 + [C.c_float] * 5 + [_I] * 2 + [c_p], _I),
     "cb200_voxel_mip_block": ([], _I),
     "cb200_voxel_mip_stride": ([c_p, _I], C.c_int64),
     "cb200_voxel_build_mip": ([C.POINTER(VoxelSet), c_p], _I),

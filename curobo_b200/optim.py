@@ -12,6 +12,10 @@ wolfe kernel -> LBFGS kernel + torch glue).
   LBFGSOpt.optimize       <- optim/gradient/lbfgs.py:157-240 + optim/components/gradient_opt_core.py:290-400 with
                              line_search_type approx_wolfe, CUDA-kernel step direction and line search
                              (content/configs/task/ik/lbfgs_ik.yml)
+  MPPIOpt.optimize        <- optim/particle/mppi.py + optim/components/particle_opt_core.py:283-441 (DIAG_A, CLAMP,
+                             content/configs/task/ik/particle_ik.yml): per inner iteration cb200_mppi_sample -> cost-only
+                             rollout -> cb200_mppi_update, where the reference runs ~20 torch launches around its rollout
+  MultiStageOpt           <- optim/multi_stage_optimizer.py:96-180 (MPPI then L-BFGS: the reference's default IK)
 
 CUDA only; no CPU path.
 """
@@ -207,3 +211,169 @@ class LBFGSOpt:
         self._graph_x0.copy_(x0.reshape(self.B, self.V))
         self._graph.replay()
         return self.best_action.view(self.B, self.H, self.D)
+
+
+def _capture_solve(owner, x0: torch.Tensor, shape: Tuple[int, ...]) -> torch.Tensor:
+    """`owner.optimize` as one CUDA graph, replayed on every call with x0 copied into the captured input (the scheme of
+    LBFGSOpt.optimize_graphed: one eager warm-up solve on the same buffers, then the capture).  Every buffer the solve
+    touches is owned by `owner`'s stages or their cost functions' engines, so the replay allocates nothing."""
+    if getattr(owner, "_graph", None) is None:
+        owner._graph_x0 = torch.empty(shape, device=owner.device, dtype=torch.float32)
+        owner._graph_x0.copy_(x0.reshape(shape))
+        owner._graph_out = owner.optimize(owner._graph_x0)            # eager warm-up, same buffers
+        torch.cuda.synchronize(owner.device)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.device(owner.device), torch.cuda.graph(g):
+            owner._graph_out = owner.optimize(owner._graph_x0)
+        owner._graph = g
+    owner._graph_x0.copy_(x0.reshape(shape))
+    owner._graph.replay()
+    return owner._graph_out
+
+
+@dataclass
+class MPPIOptCfg:
+    """The fields of MPPICfg (optim/particle/mppi.py:64-127) this loop uses; defaults = content/configs/task/ik/particle_ik.yml.
+    Supported: DIAG_A covariance, CLAMP squash, BEST or MEAN sample mode, fixed or cycling sample sets."""
+    num_iters: int = 4
+    inner_iters: int = 4
+    num_particles: int = 25
+    init_cov: float = 1.0
+    beta: float = 1.0
+    kappa: float = 0.01
+    step_size_mean: float = 0.9
+    step_size_cov: float = 0.2
+    gamma: float = 1.0
+    null_act_frac: float = 0.0
+    sample_mode: str = "BEST"
+    update_cov: bool = True
+    fixed_samples: bool = True
+    sample_per_problem: bool = True
+    seed: int = 0
+    cov_type: str = "DIAG_A"
+    squash_fn: str = "CLAMP"
+    random_mean: bool = False
+
+
+def mppi_particle_counts(num_particles: int, null_act_frac: float) -> Tuple[int, int, int]:
+    """(sampled, negated-mean, zero) particles per problem, ParticleOptCore._init_particle_counts (particle_opt_core.py:190-203)."""
+    n_null = round(int(null_act_frac * num_particles * 0.5))
+    n_neg = round(int(null_act_frac * num_particles)) - n_null
+    return num_particles - n_null - n_neg, n_neg, n_null
+
+
+class MPPIOpt:
+    """Batched MPPI over `num_problems` independent problems, three launches per inner iteration:
+
+        cb200_mppi_sample  ->  cost_fn (the cost-only fused rollout)  ->  cb200_mppi_update
+
+    `cost_fn(actions [P * Np, H, D]) -> cost [P * Np, H]`: rows are problem-major, particle-minor.  `noise`
+    [n_sets, P or 1, Ns, H, D] (n_sets = 1 with fixed samples, else num_iters; 1 problem = one set shared by every problem)
+    is copied into this object's buffer and the last sampled particle of every set is zeroed, as
+    GaussianDistribution.initialize_samples does; the default is seeded torch normal noise (the reference's scrambled-Halton
+    sample library is not reproduced).  Noise set k mod n_sets is used at global inner iteration k.
+
+    In BEST mode the result is the best particle of the LAST inner iteration of the last outer iteration -- the reference's
+    rule (mppi.py:214-218, particle_opt_core.py:464-465) -- not the best particle seen during the solve."""
+
+    def __init__(self, cfg: MPPIOptCfg, num_problems: int, action_horizon: int, action_dim: int,
+                 lows: torch.Tensor, highs: torch.Tensor, cost_fn: Callable[[torch.Tensor], torch.Tensor],
+                 noise: Optional[torch.Tensor] = None, device="cuda:0"):
+        if cfg.cov_type != "DIAG_A":
+            raise ValueError(f"MPPIOpt supports cov_type DIAG_A only, got {cfg.cov_type}")
+        if cfg.sample_mode not in ("BEST", "MEAN"):
+            raise ValueError(f"MPPIOpt supports sample_mode BEST or MEAN, got {cfg.sample_mode}")
+        if cfg.random_mean:
+            raise ValueError("MPPIOpt does not support random_mean; the mean is updated from the weighted samples")
+        if cfg.squash_fn != "CLAMP":
+            raise ValueError(f"MPPIOpt supports squash_fn CLAMP only, got {cfg.squash_fn}")
+        if cfg.num_iters < 1 or cfg.inner_iters < 1 or not cfg.beta > 0.0:
+            raise ValueError("num_iters and inner_iters must be >= 1 and beta > 0")
+        self.cfg, self.device = replace(cfg), torch.device(device)
+        _tc.require_cuda(self.device, "MPPIOpt is CUDA-only")
+        self.P, self.H, self.D, self.Np = num_problems, action_horizon, action_dim, cfg.num_particles
+        self.Ns, self.n_neg, self.n_null = mppi_particle_counts(cfg.num_particles, cfg.null_act_frac)
+        if self.Ns < 1:
+            raise ValueError("null_act_frac leaves no sampled particle")
+        P, H, D, dev = self.P, self.H, self.D, self.device
+        self.n_sets = 1 if cfg.fixed_samples else cfg.num_iters
+        shape = (self.n_sets, P if cfg.sample_per_problem else 1, self.Ns, H, D)
+        if noise is None:
+            gen = torch.Generator().manual_seed(cfg.seed)
+            noise = torch.randn(shape, generator=gen, dtype=torch.float32)
+        if tuple(noise.shape) != shape:
+            raise ValueError(f"noise must be {shape}, got {tuple(noise.shape)}")
+        self.noise = noise.to(dev, torch.float32).clone().contiguous()
+        self.noise[:, :, -1] = 0.0
+        self.lows = lows.to(dev, torch.float32).reshape(-1).contiguous()
+        self.highs = highs.to(dev, torch.float32).reshape(-1).contiguous()
+        if self.lows.numel() != D or self.highs.numel() != D:
+            raise ValueError(f"lows / highs must have {D} entries")
+        gamma_seq = torch.cumprod(torch.tensor([1.0] + [cfg.gamma] * (H - 1), dtype=torch.float32), 0)
+        self.discount = float(gamma_seq.sum() / gamma_seq[0])
+        self.cost_fn = cost_fn
+        z = lambda *s: torch.zeros(s, device=dev, dtype=torch.float32)  # noqa: E731
+        self.mean, self.best, self.action = z(P, H, D), z(P, H, D), z(P, H, D)
+        self.cov, self.scale = z(P, D), z(P, D)
+        self.actions = z(P, self.Np, H, D)
+        self.outer_iters = -(-cfg.num_iters // cfg.inner_iters)
+
+    def step(self, k: int) -> None:
+        """One inner iteration with noise set k mod n_sets: sample, evaluate, update."""
+        cfg, P, Np, H, D = self.cfg, self.P, self.Np, self.H, self.D
+        optimization_cu.launch_mppi_sample(self.actions, self.mean, self.scale, self.noise[k % self.n_sets], self.lows,
+                                           self.highs, self.n_neg)
+        cost = self.cost_fn(self.actions.view(P * Np, H, D))
+        upd = cfg.update_cov
+        optimization_cu.launch_mppi_update(self.actions, cost, self.mean, self.cov if upd else None, self.scale if upd else None,
+                                           self.best if cfg.sample_mode == "BEST" else None, cfg.beta, cfg.step_size_mean,
+                                           cfg.step_size_cov, cfg.kappa, self.discount)
+
+    def optimize(self, x0: torch.Tensor) -> torch.Tensor:
+        """ParticleOptCore.optimize / _opt_iters (particle_opt_core.py:283-388) after reinitialize: the covariance is reset to
+        init_cov and the sample index to 0; each outer iteration seeds mean and best with the current action, runs
+        inner_iters x (sample, cost_fn, update) and takes best (BEST) or mean (MEAN) as the action.  Returns [P, H, D]."""
+        cfg = self.cfg
+        self.cov.fill_(cfg.init_cov)
+        torch.sqrt(self.cov, out=self.scale)
+        self.action.copy_(x0.reshape(self.P, self.H, self.D))
+        k = 0
+        for _ in range(self.outer_iters):
+            self.mean.copy_(self.action)
+            self.best.copy_(self.action)
+            for _ in range(cfg.inner_iters):
+                self.step(k)
+                k += 1
+            self.action.copy_(self.best if cfg.sample_mode == "BEST" else self.mean)
+        return self.action
+
+    def optimize_graphed(self, x0: torch.Tensor) -> torch.Tensor:
+        """The whole stage as ONE CUDA-graph launch, as LBFGSOpt.optimize_graphed; `cost_fn` must launch on the current
+        stream and must not synchronise (RolloutEngine.evaluate_cost does neither)."""
+        return _capture_solve(self, x0, (self.P, self.H, self.D))
+
+
+class MultiStageOpt:
+    """Stages run in sequence, each seeded with the previous stage's best action (MultiStageOptimizer._opt_iters,
+    optim/multi_stage_optimizer.py:96-180): MultiStageOpt([MPPIOpt(...), LBFGSOpt(...)]) is the reference's default two-stage
+    IK.  Every stage must solve the same number of problems over the same action shape."""
+
+    def __init__(self, stages: List):
+        if not stages:
+            raise ValueError("MultiStageOpt needs at least one stage")
+        shapes = {(getattr(s, "P", getattr(s, "B", None)), s.H, s.D) for s in stages}
+        if len(shapes) != 1:
+            raise ValueError(f"stages disagree on (problems, horizon, action_dim): {sorted(shapes)}")
+        self.stages = list(stages)
+        self.shape = shapes.pop()
+        self.device = stages[0].device
+
+    def optimize(self, x0: torch.Tensor) -> torch.Tensor:
+        x = x0.reshape(self.shape)
+        for s in self.stages:
+            x = s.optimize(x).view(self.shape)
+        return x
+
+    def optimize_graphed(self, x0: torch.Tensor) -> torch.Tensor:
+        """Every stage in ONE CUDA graph: MPPI followed by L-BFGS is one launch."""
+        return _capture_solve(self, x0, self.shape)

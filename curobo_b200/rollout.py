@@ -53,6 +53,15 @@ class RolloutConfig:
                    cspace_activation=(0.01, 0.01, 0, 0, 0))
 
     @classmethod
+    def particle_ik(cls) -> "RolloutConfig":
+        """content/configs/task/ik/particle_ik.yml:3-32, the weights of the MPPI stage of the reference's two-stage IK.
+        Fields of that file RolloutConfig cannot express, at their values there: tool_pose_cfg._project_distance_to_goal
+        (false), tool_pose_cfg._terminal_pose_convergence_tolerance ([1e-8, 1e-8]), tool_pose_cfg.use_grad_input (false);
+        scene_collision_cfg.use_sweep (false) is `use_sweep`."""
+        return cls(self_weight=50.0, scene_weight=500.0, scene_activation=0.01, pose_weight=(1000.0, 10.0),
+                   cspace_type="position", cspace_weight=(50.0, 1.0, 0, 0, 0), cspace_activation=(0.001, 0.001, 0, 0, 0))
+
+    @classmethod
     def trajopt(cls) -> "RolloutConfig":
         """content/configs/task/trajopt/lbfgs_bspline_trajopt.yml:40-90."""
         return cls(self_weight=10000.0, scene_weight=100000.0, scene_activation=0.0025, use_sweep=True,

@@ -481,6 +481,33 @@ int cb200_line_search(
     cb200_stream_t stream);
 
 /* -------------------------------------------------------------------------------------------
+ * MPPI particle stage (DIAG_A covariance, CLAMP squash): the two launches either side of the cost-only rollout in
+ * every inner iteration of the reference's MPPI (optim/particle/mppi.py, optim/components/particle_opt_core.py).
+ *   cb200_mppi_sample  <- ParticleOptCore.sample_actions (particle_opt_core.py:409-441)
+ *       actions [P, Np, H, D]: per problem num_sampled particles mean + noise * scale, then num_neg copies of -mean, then
+ *       zeros; every element clamped to max(min(a, highs[d]), lows[d]).  mean [P, H, D], scale [P, D] (the DIAG_A
+ *       scale_tril), noise [P, num_sampled, H, D], or [1, num_sampled, H, D] shared by every problem when
+ *       noise_per_problem == 0; lows / highs [D].  Bit-equal to the reference's torch (mul, then add).
+ *   cb200_mppi_update  <- MPPI._update_distribution + jit_mean_cov_diag_a (mppi.py:200-248, 722-757), in place
+ *       cost [P * Np, H] (the cost-only rollout's per-row cost); total = discount * sum_h cost, discount =
+ *       sum_h gamma^h / gamma^0 (the reference broadcasts gamma_seq over the horizon-summed cost);
+ *       w = softmax(-total / beta); when best_mode, best [P, H, D] = the particle of largest w (lowest index on ties);
+ *       when update_cov, cov [P, D] = (1 - step_size_cov) cov + step_size_cov mean_h sum_p w (a - mean_old)^2 + kappa
+ *       and scale = sqrt(cov); mean = (1 - step_size_mean) mean + step_size_mean sum_p w a.
+ *       Np + H * D <= 12288.  Sums run in a fixed order: repeated calls are bit-identical.
+ * num_problems == 0 launches nothing; bad sizes or null pointers return cudaErrorInvalidValue.
+ * ------------------------------------------------------------------------------------------- */
+int cb200_mppi_sample(
+    float *actions, const float *mean, const float *scale, const float *noise, const float *lows,
+    const float *highs, int num_problems, int num_particles, int num_sampled, int num_neg, int horizon,
+    int action_dim, int noise_per_problem, cb200_stream_t stream);
+
+int cb200_mppi_update(
+    const float *actions, const float *cost, float *mean, float *cov, float *scale, float *best,
+    int num_problems, int num_particles, int horizon, int action_dim, float beta, float step_size_mean,
+    float step_size_cov, float kappa, float discount, int update_cov, int best_mode, cb200_stream_t stream);
+
+/* -------------------------------------------------------------------------------------------
  * (8f-3) RNEA inverse dynamics and its adjoint: tau = RNEA(q, qd, qdd [, f_ext]) feeds the effort terms of the STATE
  * c-space cost; the adjoint maps d loss / d tau back to (q, qd, qdd).
  *   cb200_rnea_forward   <- launch_rnea_forward   curobo/_src/curobolib/backends/cuda_core_backend/dynamics.py:24-131
