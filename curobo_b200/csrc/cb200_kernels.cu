@@ -78,6 +78,10 @@ struct FusedArgs {
   // mesh obstacles (read by the SCENE & 4 builds only).  Last member, so the parameter offsets of the members above -- and the
   // code of the builds without meshes -- do not depend on it.
   MeshSet meshes;
+  // current state of the POSITION c-space cost (velocity-aware IK): rows [n_cur, D], row index per seed (null = row 0), dt per
+  // row; cur_pos == null turns the block off, cur_vel == null reads as zero velocity
+  const float *cur_pos, *cur_vel, *cur_dt;
+  const int32_t *cur_idx;
 };
 
 // link-frame sphere set of seed b: the blob's (shared memory) unless the caller passed several configurations
@@ -154,6 +158,54 @@ __device__ __forceinline__ float seed_dt(const FusedArgs &a, int b) {
   return a.dt ? __ldg(a.dt + b) : 1.0f;
 }
 
+// POSITION c-space cost of one dof with the current-state block (wp_cspace_position.py:299-356), in the order of
+// cspace_position_kernel: shrink the bounds by the activation distance, intersect them with the window one step of dt reaches
+// from the current position, hinge with activation 0, target term, then the implied velocity / acceleration regularizers with
+// weights retimed by dt and dt^2.  Every waypoint of seed b reads the same current state.  A row whose dt <= 0 takes the plain
+// hinge of cspace_dof.  Returns the cost and d cost / d q.  Out of line: the builds that run without a current state keep their
+// register allocation.
+struct CostGrad {
+  float cost, grad;
+};
+__device__ __noinline__ CostGrad cspace_position_current(const FusedArgs &a, const float *lim, int b, int h, int d, int D,
+                                                       float qd) {
+  const cb200_rollout_cfg &c = a.cfg;
+  float cost = 0.0f, gp = 0.0f;
+  const int cur = a.cur_idx != nullptr ? __ldg(a.cur_idx + b) : 0;
+  const float dt = __ldg(a.cur_dt + cur);
+  if (!(dt > 0.0f)) {
+    bound_cost(qd, lim[d], lim[D + d], c.cspace_activation[0], c.cspace_weight[0], cost, gp);
+    cspace_target_term(a, b, h, d, D, qd, cost, gp);
+    return CostGrad{cost, gp};
+  }
+  float lo = lim[d], hi = lim[D + d];
+  {
+    const float eta = c.cspace_activation[0], r = hi - lo;
+    lo = lo + eta * r;
+    hi = hi - eta * r;
+  }
+  const float cur_p = __ldg(a.cur_pos + (size_t)cur * D + d);
+  lo = fmaxf(lo, cur_p + lim[2 * D + d] * dt);
+  hi = fminf(hi, cur_p + lim[3 * D + d] * dt);
+  bound_cost(qd, lo, hi, 0.0f, c.cspace_weight[0], cost, gp);  // an empty window (lo > hi) hinges on both sides
+  cspace_target_term(a, b, h, d, D, qd, cost, gp);
+  const float vw = c.cspace_reg[0] * dt, aw = c.cspace_reg[1] * dt * dt;
+  if (vw > 0.0f || aw > 0.0f) {
+    const float vi = (qd - cur_p) / dt;
+    if (vw > 0.0f) {
+      cost += 0.5f * vw * vi * vi;
+      gp += vw * vi / dt;
+    }
+    if (aw > 0.0f) {
+      const float cur_v = a.cur_vel != nullptr ? __ldg(a.cur_vel + (size_t)cur * D + d) : 0.0f;
+      const float ai = (vi - cur_v) / dt;
+      cost += 0.5f * aw * ai * ai;
+      gp += aw * ai / (dt * dt);
+    }
+  }
+  return CostGrad{cost, gp};
+}
+
 // c-space cost for one dof; returns cost, writes gradient wrt position into gp (and v/a/j grads to global unless !GRAD)
 template <bool GRAD = true>
 __device__ __forceinline__ float cspace_dof(const FusedArgs &a, const RobotView &rv, int e, int b, int h, int d,
@@ -165,8 +217,14 @@ __device__ __forceinline__ float cspace_dof(const FusedArgs &a, const RobotView 
   float cost = 0.0f;
   gp = 0.0f;
   if (c.cspace_type == 1) {
-    bound_cost(qd, lim[d], lim[D + d], c.cspace_activation[0], c.cspace_weight[0], cost, gp);
-    cspace_target_term(a, b, h, d, D, qd, cost, gp);
+    if (a.cur_pos != nullptr) {
+      const CostGrad r = cspace_position_current(a, lim, b, h, d, D, qd);
+      cost = r.cost;
+      gp = r.grad;
+    } else {
+      bound_cost(qd, lim[d], lim[D + d], c.cspace_activation[0], c.cspace_weight[0], cost, gp);
+      cspace_target_term(a, b, h, d, D, qd, cost, gp);
+    }
   } else if (c.cspace_type == 2) {
     const size_t idx = (size_t)e * D + d;
     const float dt = seed_dt(a, b);
@@ -2746,6 +2804,15 @@ static int prepare_rollout(const cb200_rollout_cfg *cfg, const cb200_rollout_io 
     a.cs_target = io->cspace_target;
     a.cs_target_idx = io->idxs_cspace_target;
     a.cs_target_dofw = io->cspace_target_dof_weight;
+  }
+  if (io->current_position != nullptr) {
+    if (io->current_state_dt == nullptr) return ret(cudaErrorInvalidValue);
+    if (cfg->cspace_type == 1) {  // only the POSITION cost has a current-state block
+      a.cur_pos = io->current_position;
+      a.cur_vel = io->current_velocity;
+      a.cur_idx = io->idxs_current_state;
+      a.cur_dt = io->current_state_dt;
+    }
   }
   if (io->sphere_configs != nullptr && io->num_sphere_configs > 1) {
     // the broad-phase bounds in the blob must cover every configuration

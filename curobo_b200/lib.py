@@ -73,7 +73,8 @@ class RolloutIO(C.Structure):
                 ("dynamics", C.POINTER(DynamicsParams)),
                 ("cspace_target", c_p), ("idxs_cspace_target", c_p), ("cspace_target_dof_weight", c_p),
                 ("sphere_configs", c_p), ("num_sphere_configs", C.c_int32), ("work_counter", c_p),
-                ("meshes", C.POINTER(MeshSet))]
+                ("meshes", C.POINTER(MeshSet)),
+                ("current_position", c_p), ("current_velocity", c_p), ("idxs_current_state", c_p), ("current_state_dt", c_p)]
 
 
 _I = C.c_int

@@ -62,6 +62,16 @@ class RolloutConfig:
                    cspace_type="position", cspace_weight=(50.0, 1.0, 0, 0, 0), cspace_activation=(0.001, 0.001, 0, 0, 0))
 
     @classmethod
+    def retarget_ik(cls) -> "RolloutConfig":
+        """content/configs/task/ik/lbfgs_retarget_ik.yml:3-38, the local IK of motion retargeting: with a current state
+        (RolloutEngine.update_current_state) the POSITION cost limits each step to the velocity window and regularizes the
+        implied velocity and acceleration with `cspace_reg[0]` / `cspace_reg[1]`.  The file's pose convergence tolerance
+        (1e-8, 1e-8) is update_goal(terminal_tol=...)."""
+        return cls(self_weight=10000.0, scene_weight=10000.0, scene_activation=0.0, pose_weight=(1000.0, 100.0),
+                   cspace_type="position", cspace_weight=(10000.0, 0.0, 0, 0, 0), cspace_activation=(0.01, 0.01, 0, 0, 0),
+                   cspace_reg=(0.01, 0.01, 0, 0, 0))
+
+    @classmethod
     def trajopt(cls) -> "RolloutConfig":
         """content/configs/task/trajopt/lbfgs_bspline_trajopt.yml:40-90."""
         return cls(self_weight=10000.0, scene_weight=100000.0, scene_activation=0.0025, use_sweep=True,
@@ -158,6 +168,7 @@ class RolloutEngine:
         if robot.link_spheres.ndim == 3 and robot.link_spheres.shape[0] > 1:
             self._sphere_cfgs = torch.from_numpy(np.ascontiguousarray(robot.link_spheres, np.float32)).to(self.device)
         self._cs_target = None
+        self._current_state = None
         self.cuboid, self.voxel, self.mesh = cuboid, voxel, mesh
         self.use_voxel_mip = use_voxel_mip
         self.refresh_world()
@@ -252,6 +263,38 @@ class RolloutEngine:
             if tuple(dof_weight.shape) != (D,):
                 raise ValueError(f"cspace_target_dof_weight must be [{D}]")
         self._cs_target = (target, idxs_target, dof_weight)
+
+    def update_current_state(self, position: torch.Tensor, velocity: Optional[torch.Tensor] = None,
+                             dt: Optional[torch.Tensor] = None, idxs: Optional[torch.Tensor] = None) -> None:
+        """Current state of the POSITION c-space cost (velocity-aware IK; GoalRegistry.current_js / idxs_current_js /
+        current_state_dt, cost/wp_cspace_position.py:299-356): `position` [n, D], `velocity` [n, D] (None = zero), `dt` [n]
+        (required), `idxs` [B] int32 rows per seed (None = row 0), every entry in [0, n): like idxs_cspace_target, the indices are not
+        range-checked on the device (reading them back would synchronise), and an index outside the rows reads past the buffers.  Rows with dt > 0 bound every waypoint of their seeds to
+        the window one step of dt reaches from `position` and add the implied velocity / acceleration regularizers
+        (cfg.cspace_reg[0], cfg.cspace_reg[1]); rows with dt <= 0 get the plain bound.  The tensors are read at every call,
+        so updating them in place needs no CUDA-graph recapture.  Other c-space types ignore the current state."""
+        dev, D = self.device, self.robot.num_dof
+        if dt is None:
+            raise ValueError("update_current_state needs dt [n] (current_state_dt)")
+        check_tensors(dev, torch.float32, current_position=position, current_state_dt=dt)
+        if position.ndim != 2 or position.shape[1] != D:
+            raise ValueError(f"current position must be [n, {D}], got {tuple(position.shape)}")
+        n = position.shape[0]
+        if tuple(dt.shape) != (n,):
+            raise ValueError(f"current_state_dt must be [{n}], got {tuple(dt.shape)}")
+        if velocity is not None:
+            check_tensors(dev, torch.float32, current_velocity=velocity)
+            if tuple(velocity.shape) != (n, D):
+                raise ValueError(f"current velocity must be [{n}, {D}], got {tuple(velocity.shape)}")
+        if idxs is not None:
+            check_tensors(dev, torch.int32, idxs_current_state=idxs)
+            if idxs.ndim != 1:
+                raise ValueError("idxs_current_state must be [B]")
+        self._current_state = (position, velocity, dt, idxs)
+
+    def clear_current_state(self) -> None:
+        """Back to the plain POSITION cost (no velocity window, no regularizers)."""
+        self._current_state = None
 
     def setup_batch_tensors(self, batch: int, horizon: int) -> None:
         """Allocate every output once per (B, H) -- never inside evaluate_action."""
@@ -488,6 +531,15 @@ class RolloutEngine:
                 io.idxs_cspace_target = tidx.data_ptr()
             if tdw is not None:
                 io.cspace_target_dof_weight = tdw.data_ptr()
+        if self._current_state is not None and self.cfg.cspace_type == "position":
+            cp, cv, cdt, cidx = self._current_state
+            if cidx is not None and cidx.shape[0] != B:
+                raise ValueError("idxs_current_state must have one entry per batch row")
+            io.current_position, io.current_state_dt = cp.data_ptr(), cdt.data_ptr()
+            if cv is not None:
+                io.current_velocity = cv.data_ptr()
+            if cidx is not None:
+                io.idxs_current_state = cidx.data_ptr()
         if self._sphere_cfgs is not None:
             io.sphere_configs, io.num_sphere_configs = self._sphere_cfgs.data_ptr(), int(self._sphere_cfgs.shape[0])
         io.cost = o.cost.data_ptr()

@@ -369,10 +369,38 @@ class B200RobotRollout:
                       env_query_idx: Optional[torch.Tensor] = None, state: Optional[JointState] = None,
                       start_state: Optional[JointState] = None, goal_state: Optional[JointState] = None,
                       start_state_idx: Optional[torch.Tensor] = None, goal_state_idx: Optional[torch.Tensor] = None,
-                      use_implicit_goal_state: Optional[torch.Tensor] = None, **pose_extra) -> bool:
+                      use_implicit_goal_state: Optional[torch.Tensor] = None, current_js: Optional[JointState] = None,
+                      idxs_current_js: Optional[torch.Tensor] = None, current_state_dt: Optional[torch.Tensor] = None,
+                      **pose_extra) -> bool:
         """Targets of the next solve: tool-pose goals (GoalRegistry rows: goal_* [G, L, n_goalset, 3|4], idxs_goal [B]),
         the c-space target, the world index per seed, and -- bspline and position_clique action spaces -- the boundary
-        states of the trajectory."""
+        states of the trajectory.  `current_js` (position [n, D], optional velocity), `idxs_current_js` [B] and
+        `current_state_dt` [n] (GoalRegistry's fields) are the current state of the POSITION c-space cost
+        (RolloutEngine.update_current_state); `current_state_dt` defaults to `current_js.dt`, as in the reference.  A dt of one
+        element (a float, a 0-d or [1] tensor) applies to every row; it is expanded into a tensor of this rollout, so later
+        in-place writes to the caller's scalar need another update_params.  `idxs_current_js` has one entry per evaluated row
+        (the line-search-expanded batch, like `idxs_goal`), int32 (other integer types are converted, a copy) and every entry
+        in [0, n)."""
+        if current_js is not None:
+            dt = current_state_dt if current_state_dt is not None else current_js.dt
+            if dt is None:
+                raise ValueError("current_js needs current_state_dt (or current_js.dt)")
+            pos = current_js.position
+            pos = pos.view(1, -1) if pos.ndim == 1 else pos
+            vel = current_js.velocity
+            if vel is not None and vel.ndim == 1:
+                vel = vel.view(1, -1)
+            n = pos.shape[0]
+            if not isinstance(dt, torch.Tensor):
+                dt = torch.full((n,), float(dt), dtype=torch.float32, device=self.device)
+            elif dt.numel() == 1 and n != 1:
+                dt = dt.reshape(1).to(torch.float32).expand(n).contiguous()
+            else:
+                dt = dt.reshape(-1)
+            idx = idxs_current_js
+            if idx is not None and idx.dtype != torch.int32 and not idx.is_floating_point():
+                idx = idx.to(torch.int32)
+            self.engine.update_current_state(pos, vel, dt, idx)
         if goal_position is not None:
             self.engine.update_goal(goal_position, goal_quat, idxs_goal, **pose_extra)
         if cspace_target is not None:

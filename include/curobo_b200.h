@@ -356,6 +356,20 @@ typedef struct {
    * with the arithmetic of cb200_sphere_mesh_collision.  The in-kernel B-spline schedule and `dynamics` have no mesh support:
    * with meshes present they return cudaErrorInvalidValue (the expanded spline schedule supports meshes). */
   const cb200_mesh_set *meshes;
+  /* Current state of the POSITION c-space cost (velocity-aware IK, the local IK of motion retargeting;
+   * cost/wp_cspace_position.py:299-356, fed from GoalRegistry.current_js / idxs_current_js / current_state_dt).  Seed b reads
+   * row c = idxs_current_state[b]; when current_state_dt[c] > 0 every waypoint of the seed gets
+   *   - position bounds shrunk by cspace_activation[0], then intersected with what one step reaches:
+   *     [max(p_l, current_position[c] + v_l*dt), min(p_u, current_position[c] + v_u*dt)] (v_l, v_u: the blob's velocity limits),
+   *     hinged with activation 0 (an empty window hinges on both sides, as the reference does);
+   *   - 0.5*cspace_reg[0]*dt*v^2 with v = (q - current_position[c]) / dt, and
+   *   - 0.5*cspace_reg[1]*dt^2*a^2 with a = (v - current_velocity[c]) / dt.
+   * Rows whose dt <= 0, and every row when current_position is NULL, get the plain bound hinge, bit for bit.  Read by
+   * cb200_rollout_cost_grad and cb200_rollout_cost when cfg->cspace_type == 1 (POSITION); the STATE cost ignores them. */
+  const float *current_position;          /* [n_cur, D] or null (= off) */
+  const float *current_velocity;          /* [n_cur, D] or null (= 0) */
+  const int32_t *idxs_current_state;      /* [B] rows of current_position; null = row 0 */
+  const float *current_state_dt;          /* [n_cur]; required with current_position (else cudaErrorInvalidValue) */
 } cb200_rollout_io;
 
 int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io *io,
