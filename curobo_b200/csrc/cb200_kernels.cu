@@ -2022,81 +2022,49 @@ __global__ void voxel_mip_kernel(VoxelSet vs, uint16_t *mip, int n_layers) {
   }
 }
 
+// Robot-sphere refresh (cb200_refresh_robot_spheres): configuration 0 of link_spheres [n_cfg, S, 4] -> the blob's sphere section,
+// then warp w rebuilds the two broad-phase bounds of collision link w with the packer's bounding_ball.
+struct SphereRefreshArgs {
+  unsigned char *blob;
+  const float *link_spheres;
+  int32_t S, n_cfg, n_cl;
+  int32_t off_spheres, off_padding, off_cl_start, off_cl_bound, off_cl_bound_scene;
+};
+
+// bounding_ball's farthest-ball scan over a warp: the largest distance, the lowest slot among equals (the serial scan's pick)
+struct WarpFarthest {
+  __device__ void operator()(double &best, int &arg) const {
+    for (int o = 16; o > 0; o >>= 1) {
+      const double b = __shfl_xor_sync(0xffffffffu, best, o);
+      const int j = __shfl_xor_sync(0xffffffffu, arg, o);
+      if (b > best || (b == best && j < arg)) {
+        best = b;
+        arg = j;
+      }
+    }
+  }
+};
+
+__global__ void __launch_bounds__(128) refresh_robot_spheres_kernel(const SphereRefreshArgs a) {
+  const int tid = blockIdx.x * blockDim.x + threadIdx.x, nthreads = gridDim.x * blockDim.x;
+  float *spheres = reinterpret_cast<float *>(a.blob + a.off_spheres);
+  for (int i = tid; i < 4 * a.S; i += nthreads) spheres[i] = a.link_spheres[i];
+  const int cl = tid >> 5, lane = threadIdx.x & 31;
+  if (cl >= a.n_cl) return;  // whole warps
+  const int16_t *cl_start = reinterpret_cast<const int16_t *>(a.blob + a.off_cl_start);
+  const float *padding = reinterpret_cast<const float *>(a.blob + a.off_padding);
+  const int s0 = cl_start[cl], s1 = cl_start[cl + 1];
+  bounding_ball(a.link_spheres, padding, s0, s1, a.n_cfg, a.S, reinterpret_cast<float *>(a.blob + a.off_cl_bound) + 4 * cl, lane,
+                32, WarpFarthest{});
+  bounding_ball(a.link_spheres, (const float *)nullptr, s0, s1, a.n_cfg, a.S,
+                reinterpret_cast<float *>(a.blob + a.off_cl_bound_scene) + 4 * cl, lane, 32, WarpFarthest{});
+}
+
 }  // namespace
 
 // ================================================================================================
 // C ABI
 // ================================================================================================
-// Near-minimal ball enclosing the balls (p_s, r_s [+ padding_s]) of spheres [s_begin, s_end) with radius >= 0:
-// Badoiu-Clarkson iterations from the centroid (move the centre 1/(k+1) of the way towards the farthest ball), then
-// R = max(|p - c| + r) exactly for the final centre, inflated against fp32 rounding of the world transform.
-// out = (cx, cy, cz, R); R = -1 when no sphere is enabled.  A tighter ball only prunes more; it is never unsafe.
-static void bounding_ball(const float *link_spheres, const float *padding, int s_begin, int s_end, float *out, int n_cfg = 1,
-                          int S = 0) {
-  // the balls of every configuration of spheres [s_begin, s_end): (centre, radius) with radius >= 0
-  std::vector<double> bx, by, bz, br;
-  for (int c = 0; c < (n_cfg < 1 ? 1 : n_cfg); ++c) {
-    const float *ls = link_spheres + (size_t)c * S * 4;
-    for (int s = s_begin; s < s_end; ++s) {
-      const double r = (double)ls[4 * s + 3] + (padding ? (double)padding[s] : 0.0);
-      if (r < 0) continue;
-      bx.push_back(ls[4 * s]);
-      by.push_back(ls[4 * s + 1]);
-      bz.push_back(ls[4 * s + 2]);
-      br.push_back(r);
-    }
-  }
-  const int n = (int)bx.size();
-  double c[3] = {0, 0, 0};
-  out[0] = out[1] = out[2] = 0.0f;
-  out[3] = -1.0f;
-  if (n == 0) return;
-  for (int i = 0; i < n; ++i) {
-    c[0] += bx[i];
-    c[1] += by[i];
-    c[2] += bz[i];
-  }
-  for (int k = 0; k < 3; ++k) c[k] /= n;
-  auto farthest = [&](const double *cc, int &arg) {
-    double best = -1;
-    arg = -1;
-    for (int i = 0; i < n; ++i) {
-      const double dx = bx[i] - cc[0], dy = by[i] - cc[1], dz = bz[i] - cc[2];
-      const double d = std::sqrt(dx * dx + dy * dy + dz * dz) + br[i];
-      if (d > best) {
-        best = d;
-        arg = i;
-      }
-    }
-    return best;
-  };
-  int arg;
-  double best_R = farthest(c, arg), best_c[3] = {c[0], c[1], c[2]};
-  for (int it = 1; it <= 200; ++it) {
-    const double R = farthest(c, arg);
-    if (R < best_R) {
-      best_R = R;
-      for (int k = 0; k < 3; ++k) best_c[k] = c[k];
-    }
-    // step towards the farthest ball's centre, 1/(it+1) of the current radius, never past the centre
-    const double dx = bx[arg] - c[0], dy = by[arg] - c[1], dz = bz[arg] - c[2];
-    const double d = std::sqrt(dx * dx + dy * dy + dz * dz);
-    if (d < 1e-12) break;
-    const double mv = std::min(R / (it + 1.0), d) / d;
-    c[0] += dx * mv;
-    c[1] += dy * mv;
-    c[2] += dz * mv;
-  }
-  const double Rf = farthest(best_c, arg);
-  out[0] = (float)best_c[0];
-  out[1] = (float)best_c[1];
-  out[2] = (float)best_c[2];
-  // centre was rounded to fp32: re-measure from the rounded centre
-  double cr[3] = {(double)out[0], (double)out[1], (double)out[2]};
-  const double Rr = farthest(cr, arg);
-  out[3] = (float)(std::max(Rf, Rr) * (1.0 + 1e-4) + 1e-5);
-}
-
 // which kernel the last cb200_rollout_cost_grad / cb200_rollout_cost call of this thread launched (CB200_VARIANT_*; test / bench introspection)
 static thread_local int g_last_variant = 0;
 
@@ -2572,9 +2540,9 @@ int64_t cb200_pack_robot_blob(void *out, int64_t out_bytes, const cb200_robot_si
         cll[a] = (int16_t)cl_link[a];
         cls[a] = (int16_t)cl_start[a];
         // bounding spheres of the enabled sphere balls: padded radii for self collision, raw radii for the scene
-        bounding_ball(link_spheres, sphere_padding, cl_start[a], cl_start[a + 1], clb + 4 * a, n_cfg, S);
-        bounding_ball(link_spheres, nullptr, cl_start[a], cl_start[a + 1],
-                      reinterpret_cast<float *>(o + h.off_cl_bound_scene) + 4 * a, n_cfg, S);
+        bounding_ball(link_spheres, sphere_padding, cl_start[a], cl_start[a + 1], n_cfg, S, clb + 4 * a);
+        bounding_ball(link_spheres, nullptr, cl_start[a], cl_start[a + 1], n_cfg, S,
+                      reinterpret_cast<float *>(o + h.off_cl_bound_scene) + 4 * a);
       }
       cls[n_cl] = (int16_t)S;
       memcpy(o + h.off_lp, lps.data(), lps.size() * 4);
@@ -2582,6 +2550,24 @@ int64_t cb200_pack_robot_blob(void *out, int64_t out_bytes, const cb200_robot_si
     }
   }
   return total;
+}
+
+int cb200_refresh_robot_spheres(void *robot_blob, const void *robot_blob_host, int32_t robot_blob_bytes, const float *link_spheres,
+                                int32_t num_sphere_configs, cb200_stream_t stream) {
+  CB200_DEVICE_GUARD(robot_blob);
+  if (robot_blob == nullptr || robot_blob_host == nullptr || link_spheres == nullptr ||
+      robot_blob_bytes < (int32_t)sizeof(BlobHeader))
+    return ret(cudaErrorInvalidValue);
+  BlobHeader h;
+  memcpy(&h, robot_blob_host, sizeof(BlobHeader));
+  if (h.magic != kBlobMagic || h.total_bytes != robot_blob_bytes || num_sphere_configs != h.n_sphere_cfgs)
+    return ret(cudaErrorInvalidValue);
+  if (h.S == 0) return ret(cudaSuccess);
+  const SphereRefreshArgs a{static_cast<unsigned char *>(robot_blob), link_spheres, h.S, h.n_sphere_cfgs, h.n_cl, h.off_spheres,
+                            h.off_padding, h.off_cl_start, h.off_cl_bound, h.off_cl_bound_scene};
+  const int grid = std::max(1, (h.n_cl * 32 + 127) / 128);  // a warp per collision link (none when n_lp == 0: n_cl == 0)
+  CB200_LAUNCH(refresh_robot_spheres_kernel, grid, 128, 0, (cudaStream_t)stream, a);
+  return launch_status();
 }
 
 }  // extern "C"

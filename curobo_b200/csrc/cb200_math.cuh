@@ -713,4 +713,118 @@ CB_HD void l2_reg(float v, float w, float &cost, float &grad) {
   grad += wv;
 }
 
+// ----------------------------------------------------------------------------------------------
+// Broad-phase bound of a collision link: the blob packer (host) and cb200_refresh_robot_spheres (device) both call
+// bounding_ball, so a refreshed blob holds the bytes a fresh pack would.
+// ----------------------------------------------------------------------------------------------
+// fp64 spelled, on the device, with round-to-nearest operations: nvcc cannot contract them into FMAs, so the device rounds every
+// step exactly as the host code (x86-64 without FMA, also the host emulation of the kernels) does.
+#ifdef __CUDA_ARCH__
+CB_HD double bb_add(double a, double b) { return __dadd_rn(a, b); }
+CB_HD double bb_sub(double a, double b) { return __dsub_rn(a, b); }
+CB_HD double bb_mul(double a, double b) { return __dmul_rn(a, b); }
+CB_HD double bb_div(double a, double b) { return __ddiv_rn(a, b); }
+CB_HD double bb_sqrt(double a) { return __dsqrt_rn(a); }
+#else
+CB_HD double bb_add(double a, double b) { return a + b; }
+CB_HD double bb_sub(double a, double b) { return a - b; }
+CB_HD double bb_mul(double a, double b) { return a * b; }
+CB_HD double bb_div(double a, double b) { return a / b; }
+CB_HD double bb_sqrt(double a) { return sqrt(a); }
+#endif
+
+// Ball j of the slots (configuration j / m, sphere s_begin + j % m) of link_spheres [n_cfg, S, 4]: centre and radius
+// (+ padding[s] when padding is given); false when the radius is negative (a disabled sphere).
+CB_HD bool bb_ball(const float *link_spheres, const float *padding, int s_begin, int m, int S, int j, double *b) {
+  const int cfg = j / m, s = s_begin + (j - cfg * m);
+  const float *p = link_spheres + ((size_t)cfg * S + s) * 4;
+  b[3] = bb_add((double)p[3], padding ? (double)padding[s] : 0.0);
+  b[0] = p[0];
+  b[1] = p[1];
+  b[2] = p[2];
+  return !(b[3] < 0);
+}
+
+// The ball farthest from c (max |p - c| + r; the lowest slot among equals) over the slots lane, lane + nlanes, ...;
+// `reduce(best, arg)` combines the lanes' candidates (nothing to combine for one lane).
+struct SerialFarthest {
+  CB_HD void operator()(double &, int &) const {}
+};
+template <class Reduce>
+CB_HD double bb_farthest(const float *ls, const float *padding, int s_begin, int m, int S, int n_slots, const double *c, int lane,
+                         int nlanes, const Reduce &reduce, int &arg) {
+  double best = -1, b[4];
+  arg = -1;
+  for (int j = lane; j < n_slots; j += nlanes) {
+    if (!bb_ball(ls, padding, s_begin, m, S, j, b)) continue;
+    const double dx = bb_sub(b[0], c[0]), dy = bb_sub(b[1], c[1]), dz = bb_sub(b[2], c[2]);
+    const double d = bb_add(bb_sqrt(bb_add(bb_add(bb_mul(dx, dx), bb_mul(dy, dy)), bb_mul(dz, dz))), b[3]);
+    if (d > best) {
+      best = d;
+      arg = j;
+    }
+  }
+  reduce(best, arg);
+  return best;
+}
+
+// Near-minimal ball enclosing the balls (p_s, r_s [+ padding_s]) with radius >= 0 of spheres [s_begin, s_end) of every
+// configuration of link_spheres [n_cfg, S, 4]: Badoiu-Clarkson iterations from the centroid (move the centre 1/(k+1) of the way
+// towards the farthest ball), then R = max(|p - c| + r) exactly for the final centre, inflated against fp32 rounding of the world
+// transform.  out = (cx, cy, cz, R), written by lane 0; R = -1 when no sphere is enabled.  A tighter ball only prunes more; it is
+// never unsafe.  Lanes 0..nlanes-1 share the farthest-ball scans through `reduce` and compute everything else redundantly.
+template <class Reduce = SerialFarthest>
+CB_HD void bounding_ball(const float *link_spheres, const float *padding, int s_begin, int s_end, int n_cfg, int S, float *out,
+                         int lane = 0, int nlanes = 1, const Reduce &reduce = Reduce()) {
+  const int m = s_end - s_begin, n_slots = (n_cfg < 1 ? 1 : n_cfg) * m;
+  double c[3] = {0, 0, 0}, b[4];
+  int n = 0;
+  for (int j = 0; j < n_slots; ++j) {
+    if (!bb_ball(link_spheres, padding, s_begin, m, S, j, b)) continue;
+    c[0] = bb_add(c[0], b[0]);
+    c[1] = bb_add(c[1], b[1]);
+    c[2] = bb_add(c[2], b[2]);
+    ++n;
+  }
+  if (n == 0) {
+    if (lane == 0) {
+      out[0] = out[1] = out[2] = 0.0f;
+      out[3] = -1.0f;
+    }
+    return;
+  }
+  for (int k = 0; k < 3; ++k) c[k] = bb_div(c[k], (double)n);
+  int arg;
+  double best_R = bb_farthest(link_spheres, padding, s_begin, m, S, n_slots, c, lane, nlanes, reduce, arg);
+  double best_c[3] = {c[0], c[1], c[2]};
+  for (int it = 1; it <= 200; ++it) {
+    const double R = bb_farthest(link_spheres, padding, s_begin, m, S, n_slots, c, lane, nlanes, reduce, arg);
+    if (R < best_R) {
+      best_R = R;
+      for (int k = 0; k < 3; ++k) best_c[k] = c[k];
+    }
+    // step towards the farthest ball's centre, 1/(it+1) of the current radius, never past the centre
+    bb_ball(link_spheres, padding, s_begin, m, S, arg, b);
+    const double dx = bb_sub(b[0], c[0]), dy = bb_sub(b[1], c[1]), dz = bb_sub(b[2], c[2]);
+    const double d = bb_sqrt(bb_add(bb_add(bb_mul(dx, dx), bb_mul(dy, dy)), bb_mul(dz, dz)));
+    if (d < 1e-12) break;
+    const double step = bb_div(R, bb_add((double)it, 1.0));
+    const double mv = bb_div(d < step ? d : step, d);
+    c[0] = bb_add(c[0], bb_mul(dx, mv));
+    c[1] = bb_add(c[1], bb_mul(dy, mv));
+    c[2] = bb_add(c[2], bb_mul(dz, mv));
+  }
+  const double Rf = bb_farthest(link_spheres, padding, s_begin, m, S, n_slots, best_c, lane, nlanes, reduce, arg);
+  const float o[3] = {(float)best_c[0], (float)best_c[1], (float)best_c[2]};
+  // centre was rounded to fp32: re-measure from the rounded centre
+  const double cr[3] = {(double)o[0], (double)o[1], (double)o[2]};
+  const double Rr = bb_farthest(link_spheres, padding, s_begin, m, S, n_slots, cr, lane, nlanes, reduce, arg);
+  if (lane == 0) {
+    out[0] = o[0];
+    out[1] = o[1];
+    out[2] = o[2];
+    out[3] = (float)bb_add(bb_mul(Rf < Rr ? Rr : Rf, 1.0 + 1e-4), 1e-5);
+  }
+}
+
 }  // namespace cb200

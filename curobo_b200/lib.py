@@ -119,6 +119,7 @@ _SIGS = {
     "cb200_tsdf_stamp_cuboids": ([c_p, _I, _I, _I, C.c_float, C.POINTER(C.c_float), C.c_float, C.POINTER(CuboidSet), _I, c_p], _I),
     "cb200_robot_blob_bytes": ([C.POINTER(RobotSizes)], C.c_int64),
     "cb200_pack_robot_blob": ([c_p, C.c_int64, C.POINTER(RobotSizes)] + [c_p] * 15, C.c_int64),
+    "cb200_refresh_robot_spheres": ([c_p, c_p, C.c_int32, c_p, C.c_int32, c_p], _I),
     "cb200_rollout_cost_grad": ([C.POINTER(RolloutCfg), C.POINTER(RolloutIO), c_p], _I),
     "cb200_rollout_cost": ([C.POINTER(RolloutCfg), C.POINTER(RolloutIO), c_p], _I),
 }

@@ -149,11 +149,34 @@ def pack_robot_blob(rm: RobotModel) -> np.ndarray:
     return out[:n]
 
 
+def _quat_mul(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """Hamilton product of wxyz quaternions [..., 4]."""
+    aw, ax, ay, az = a.unbind(-1)
+    bw, bx, by, bz = b.unbind(-1)
+    return torch.stack((aw * bw - ax * bx - ay * by - az * bz, aw * bx + ax * bw + ay * bz - az * by,
+                        aw * by - ax * bz + ay * bw + az * bx, aw * bz + ax * by - ay * bx + az * bw), -1)
+
+
+def _quat_rotate(q: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
+    """Rotate points v [..., 3] by unit wxyz quaternions q [..., 4]: v + 2 w (u x v) + 2 u x (u x v)."""
+    w, u = q[..., :1], q[..., 1:]
+    t = 2.0 * torch.linalg.cross(u, v, dim=-1)
+    return v + w * t + torch.linalg.cross(u, t, dim=-1)
+
+
 class RolloutEngine:
     """`mesh` (curobo_b200.mesh.MeshData): triangle-mesh obstacles, evaluated inside the fused kernels next to the cuboids and
     the ESDF grids.  In-place updates of its `inv_pose` / `enable` tensors take effect on the next call; a replaced MeshData
     needs refresh_world().  Mesh scenes support every schedule except `evaluate_knots(in_kernel_spline=True)` and
-    `attach_dynamics(fused=True)`, which raise ValueError."""
+    `attach_dynamics(fused=True)`, which raise ValueError.
+
+    `link_spheres` [n_cfg, S, 4] (device, float32) are the robot's collision spheres in their link frames, one set per sphere
+    configuration (rows pick theirs through env_query_idx when n_cfg > 1); `reference_link_spheres` keeps the model's.  The
+    update_link_spheres / disable_link_spheres / enable_link_spheres / reset_link_spheres / attach_object_spheres calls (the
+    reference's KinematicsParams and AttachmentManager calls) write `link_spheres` and refresh the packed robot constants on the
+    device in one launch (cb200_refresh_robot_spheres): the broad-phase bounds are rebuilt over the new spheres, so the next
+    evaluation equals, bit for bit, that of an engine built from the modified model.  The device blob keeps its address, so CUDA
+    graphs captured before an update see it on their next replay without recapture."""
 
     def __init__(self, robot: RobotModel, cfg: RolloutConfig, device="cuda:0",
                  cuboid: Optional[CuboidData] = None, voxel: Optional[VoxelData] = None,
@@ -163,10 +186,12 @@ class RolloutEngine:
         self._lib = _lib.load()
         self._blob_host = pack_robot_blob(robot)
         self._blob = torch.from_numpy(self._blob_host.copy()).to(self.device)
-        # several link-sphere configurations (attached objects per environment): rows pick theirs through env_query_idx
-        self._sphere_cfgs = None
-        if robot.link_spheres.ndim == 3 and robot.link_spheres.shape[0] > 1:
-            self._sphere_cfgs = torch.from_numpy(np.ascontiguousarray(robot.link_spheres, np.float32)).to(self.device)
+        # link-sphere configurations (attached objects per environment): rows pick theirs through env_query_idx when n_cfg > 1;
+        # configuration 0 is also the blob's staged set
+        ls = robot.link_spheres if robot.link_spheres.ndim == 3 else robot.link_spheres[None]
+        self.link_spheres = torch.from_numpy(np.ascontiguousarray(ls, np.float32)).to(self.device)
+        self.reference_link_spheres = self.link_spheres.clone()
+        self._link_spheres_version = self.link_spheres._version
         self._cs_target = None
         self._current_state = None
         self.cuboid, self.voxel, self.mesh = cuboid, voxel, mesh
@@ -226,6 +251,131 @@ class RolloutEngine:
         self._ms = c_mesh_set(self.mesh, self.device)
         if self.voxel is not None and not self.use_voxel_mip and self._vs is not None:
             self._vs.mip, self._vs.mip_stride = None, 0
+
+    # -- link spheres (KinematicsParams.update_link_spheres & co., kinematics_params.py:493-595) -----------------------------
+    def refresh_link_spheres(self) -> None:
+        """Re-read `link_spheres` into the packed robot constants on the device (one launch on the current stream: configuration
+        0 into the blob's sphere section, broad-phase bounds of every collision link rebuilt over all configurations).  The
+        methods below call it.  Eager evaluations also pick up in-place writes to `link_spheres` by themselves (version
+        stamp); a CUDA graph does not -- after writing the tensor yourself, call this before replaying, or capture this call
+        in the graph."""
+        ls = self.link_spheres
+        err = self._lib.cb200_refresh_robot_spheres(self._blob.data_ptr(), self._blob_host.ctypes.data,
+                                                    int(self._blob_host.shape[0]), ls.data_ptr(), int(ls.shape[0]),
+                                                    stream_ptr(self.device))
+        _lib.check(err, "refresh_robot_spheres")
+        self._link_spheres_version = ls._version
+
+    def _sphere_index(self, link_name: str) -> torch.Tensor:
+        """Sphere slots of `link_name` (KinematicsParams.get_sphere_index_from_link_name)."""
+        rm = self.robot
+        if link_name not in rm.link_names:
+            raise ValueError(f"unknown link {link_name!r}")
+        idx = np.nonzero(rm.link_sphere_idx_map == rm.link_names.index(link_name))[0]
+        if idx.size == 0:
+            raise ValueError(f"link {link_name!r} has no collision spheres")
+        return torch.as_tensor(idx, dtype=torch.long, device=self.device)
+
+    def _config_index(self, config_idx: int) -> int:
+        n = int(self.link_spheres.shape[0])
+        if not 0 <= int(config_idx) < n:
+            raise ValueError(f"config_idx {config_idx} out of range: the engine has {n} sphere configuration(s)")
+        return int(config_idx)
+
+    def update_link_spheres(self, link_name: str, spheres: torch.Tensor, start_sph_idx: int = 0,
+                            config_idx: Optional[int] = None) -> None:
+        """Write spheres [k, 4] (x, y, z, r in the link frame; r < 0 disables a sphere) into slots start_sph_idx ..
+        start_sph_idx + k - 1 of `link_name`, in configuration `config_idx` (None: every configuration), then refresh."""
+        idx = self._sphere_index(link_name)
+        check_tensors(self.device, torch.float32, spheres=spheres)
+        if spheres.ndim != 2 or spheres.shape[1] != 4:
+            raise ValueError(f"spheres must be [k, 4], got {tuple(spheres.shape)}")
+        k = int(spheres.shape[0])
+        if start_sph_idx < 0 or start_sph_idx + k > idx.numel():
+            raise ValueError(f"link {link_name!r} has {idx.numel()} sphere slots; cannot write {k} from slot {start_sph_idx}")
+        idx = idx[start_sph_idx:start_sph_idx + k]
+        if config_idx is None:
+            self.link_spheres[:, idx, :] = spheres
+        else:
+            self.link_spheres[self._config_index(config_idx), idx, :] = spheres
+        self.refresh_link_spheres()
+
+    def get_link_spheres(self, link_name: str, config_idx: int = 0) -> torch.Tensor:
+        """Spheres [n, 4] of `link_name` in configuration `config_idx` (a copy)."""
+        return self.link_spheres[self._config_index(config_idx), self._sphere_index(link_name), :]
+
+    def disable_link_spheres(self, link_name: str) -> None:
+        """Radius -100 for every sphere of `link_name` in every configuration (MotionPlanner.disable_link_collision)."""
+        self.link_spheres[:, self._sphere_index(link_name), 3] = -100.0
+        self.refresh_link_spheres()
+
+    def enable_link_spheres(self, link_name: str) -> None:
+        """Radii of `link_name` back to the model's in every configuration; centres are left as they are."""
+        idx = self._sphere_index(link_name)
+        self.link_spheres[:, idx, 3] = self.reference_link_spheres[:, idx, 3]
+        self.refresh_link_spheres()
+
+    def reset_link_spheres(self, link_name: str) -> None:
+        """Spheres (centres and radii) of `link_name` back to the model's in every configuration."""
+        idx = self._sphere_index(link_name)
+        self.link_spheres[:, idx, :] = self.reference_link_spheres[:, idx, :]
+        self.refresh_link_spheres()
+
+    def attach_object_spheres(self, spheres: torch.Tensor, link_name: str = "attached_object",
+                              joint_position: Optional[torch.Tensor] = None, object_pose: Optional[torch.Tensor] = None) -> None:
+        """AttachmentManager.update (collision/attachment_manager.py:102-179) as one call: spheres [k, 4] fitted to the object,
+        in the object frame, become the spheres of `link_name`, one environment per sphere configuration.
+
+        joint_position [n_env, D]: the grasp configuration of each environment; object_pose [n_env or 1, 7] (x, y, z, qw, qx, qy,
+        qz): the object's pose in the robot base frame.  With object_pose, environment i gets the centres mapped by
+        obj_to_link = ee_pose(joint_position[i])^-1 * object_pose[i], ee_pose being the first tool frame's pose from the
+        forward kinematics (joint_position is then required); without it the centres are taken as link-frame centres.  The
+        link's slots past k get radius -100 (disabled).  Environment i is written into configuration i, then the blob is
+        refreshed once.  Per-environment attachment needs an engine built with at least n_env sphere configurations (a model
+        whose link_spheres is [n_cfg, S, 4]); rows pick theirs through env_query_idx.  Sphere fitting stays with the caller."""
+        idx = self._sphere_index(link_name)
+        dev = self.device
+        check_tensors(dev, torch.float32, spheres=spheres)
+        if spheres.ndim != 2 or spheres.shape[1] != 4:
+            raise ValueError(f"spheres must be [k, 4], got {tuple(spheres.shape)}")
+        k, n_slots = int(spheres.shape[0]), int(idx.numel())
+        if k > n_slots:
+            raise ValueError(f"{k} spheres but link {link_name!r} only has {n_slots} sphere slots")
+        n_env = 1
+        if joint_position is not None:
+            check_tensors(dev, torch.float32, joint_position=joint_position)
+            if joint_position.ndim != 2 or joint_position.shape[1] != self.robot.num_dof:
+                raise ValueError(f"joint_position must be [n_env, {self.robot.num_dof}], got {tuple(joint_position.shape)}")
+            n_env = int(joint_position.shape[0])
+        if n_env > int(self.link_spheres.shape[0]):
+            raise ValueError(f"{n_env} environments but the engine has {int(self.link_spheres.shape[0])} sphere configuration(s)")
+        centres = spheres[:, :3].expand(n_env, k, 3)
+        if object_pose is not None:
+            if joint_position is None:
+                raise ValueError("object_pose needs joint_position (the grasp configuration the end-effector pose comes from)")
+            check_tensors(dev, torch.float32, object_pose=object_pose)
+            if object_pose.ndim != 2 or object_pose.shape[1] != 7 or object_pose.shape[0] not in (1, n_env):
+                raise ValueError(f"object_pose must be [{n_env} or 1, 7], got {tuple(object_pose.shape)}")
+            from .kinematics import Kinematics
+            # one sphere configuration index per row: with several configurations the FK kernel reads env_query_idx[row]
+            st = Kinematics(self.robot, dev).compute_kinematics(joint_position,
+                                                                torch.zeros(n_env, dtype=torch.int32, device=dev))
+            ee_p, ee_q = st.tool_pose_position[:, 0, 0], st.tool_pose_quaternion[:, 0, 0]       # [n_env, 3], [n_env, 4]
+            ee_qi = ee_q * torch.tensor([1.0, -1.0, -1.0, -1.0], device=dev)
+            op, oq = object_pose[:, :3].expand(n_env, 3), object_pose[:, 3:].expand(n_env, 4)
+            rel_q = _quat_mul(ee_qi, oq)
+            rel_p = _quat_rotate(ee_qi, op - ee_p)
+            centres = _quat_rotate(rel_q[:, None, :].expand(n_env, k, 4), centres) + rel_p[:, None, :]
+        env = torch.zeros((n_env, n_slots, 4), dtype=torch.float32, device=dev)
+        env[:, :, 3] = -100.0
+        env[:, :k, :3] = centres
+        env[:, :k, 3] = spheres[:, 3]
+        self.link_spheres[:n_env, idx, :] = env
+        self.refresh_link_spheres()
+
+    def detach_object_spheres(self, link_name: str = "attached_object") -> None:
+        """The attached object's spheres off again: reset_link_spheres(link_name)."""
+        self.reset_link_spheres(link_name)
 
     # -- configuration ------------------------------------------------------------------------
     def _make_ccfg(self, num_goalset: int) -> _lib.RolloutCfg:
@@ -540,8 +690,12 @@ class RolloutEngine:
                 io.current_velocity = cv.data_ptr()
             if cidx is not None:
                 io.idxs_current_state = cidx.data_ptr()
-        if self._sphere_cfgs is not None:
-            io.sphere_configs, io.num_sphere_configs = self._sphere_cfgs.data_ptr(), int(self._sphere_cfgs.shape[0])
+        if self.link_spheres._version != self._link_spheres_version:   # written in place since the last refresh
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("link_spheres changed since the last refresh; call refresh_link_spheres() before capturing")
+            self.refresh_link_spheres()
+        if self.link_spheres.shape[0] > 1:
+            io.sphere_configs, io.num_sphere_configs = self.link_spheres.data_ptr(), int(self.link_spheres.shape[0])
         io.cost = o.cost.data_ptr()
         if grad:
             io.grad_q = o.grad_q.data_ptr()

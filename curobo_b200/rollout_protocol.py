@@ -444,3 +444,36 @@ class B200RobotRollout:
 
     def refresh_world(self) -> None:
         self.engine.refresh_world()
+
+    # -- link spheres: RolloutEngine's calls (the reference's KinematicsParams / AttachmentManager); graphs captured on this
+    # rollout see an update on their next replay without recapture (the packed robot constants keep their address) -------------
+    @property
+    def link_spheres(self) -> torch.Tensor:
+        """[n_cfg, S, 4] link-frame spheres (see RolloutEngine.refresh_link_spheres for in-place writes)."""
+        return self.engine.link_spheres
+
+    def update_link_spheres(self, link_name: str, spheres: torch.Tensor, start_sph_idx: int = 0,
+                            config_idx: Optional[int] = None) -> None:
+        self.engine.update_link_spheres(link_name, spheres, start_sph_idx, config_idx)
+
+    def get_link_spheres(self, link_name: str, config_idx: int = 0) -> torch.Tensor:
+        return self.engine.get_link_spheres(link_name, config_idx)
+
+    def disable_link_spheres(self, link_name: str) -> None:
+        self.engine.disable_link_spheres(link_name)
+
+    def enable_link_spheres(self, link_name: str) -> None:
+        self.engine.enable_link_spheres(link_name)
+
+    def reset_link_spheres(self, link_name: str) -> None:
+        self.engine.reset_link_spheres(link_name)
+
+    def refresh_link_spheres(self) -> None:
+        self.engine.refresh_link_spheres()
+
+    def attach_object_spheres(self, spheres: torch.Tensor, link_name: str = "attached_object",
+                              joint_position: Optional[torch.Tensor] = None, object_pose: Optional[torch.Tensor] = None) -> None:
+        self.engine.attach_object_spheres(spheres, link_name, joint_position, object_pose)
+
+    def detach_object_spheres(self, link_name: str = "attached_object") -> None:
+        self.engine.detach_object_spheres(link_name)

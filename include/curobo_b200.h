@@ -629,6 +629,20 @@ int64_t cb200_pack_robot_blob(
     const float *position_limits, const float *velocity_limits, const float *acceleration_limits,
     const float *jerk_limits, const float *effort_limits);
 
+/* Link spheres changed after packing (KinematicsParams.update_link_spheres / disable_link_spheres / AttachmentManager.update,
+ * curobo/_src/robot/types/kinematics_params.py:493-595, collision/attachment_manager.py:102-315): one launch on `stream` copies
+ * configuration 0 of link_spheres into the DEVICE blob's sphere section and rebuilds the broad-phase bounds of every collision link
+ * (padded radii for self collision, raw radii for the scene) over the enabled spheres (r >= 0) of all configurations, with the
+ * packer's own arithmetic: the blob becomes, byte for byte, what cb200_pack_robot_blob packs from the same spheres.  Every other
+ * byte is left alone; a blob without a link-pair list (n_lp == 0) has no bounds, and only the spheres are copied.
+ * robot_blob: DEVICE blob; robot_blob_host: HOST copy (its header is read on the host, its bytes are not updated);
+ * link_spheres: DEVICE [num_sphere_configs, S, 4], num_sphere_configs equal to the configurations the blob was packed with.
+ * A null pointer, a header that is not a blob of robot_blob_bytes bytes or another configuration count return
+ * cudaErrorInvalidValue before any device work.  No allocation, no synchronisation: the call can be captured in a CUDA graph. */
+int cb200_refresh_robot_spheres(void *robot_blob, const void *robot_blob_host, int32_t robot_blob_bytes,
+                                const float *link_spheres /*[n_cfg, S, 4]*/, int32_t num_sphere_configs,
+                                cb200_stream_t stream);
+
 /* Device properties the host side sizes persistent grids with (SM count, max dynamic smem). */
 int cb200_device_info(int device, int *sm_count, int *max_smem_optin);
 
