@@ -673,6 +673,88 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, MINB) rollout_cost_kernel(c
 }
 
 // ------------------------------------------------------------------------------------------------
+// Validity rows (cb200_rollout_validate): is row (b, h) inside the position limits, free of scene contact and free of self
+// contact?  The reference's RobotSceneCollision.validate sums non-negative terms and tests the sum against 0, so each check is
+// "its term is exactly 0", asked in the order of cost: bounds (before FK), scene, self.  A row leaves at the first check that
+// fails; every exit is a warp vote (__ballot_sync) at a chunk boundary -- 32 dofs, 32 spheres, one link-pair block of the
+// self-collision scan -- so an exit changes when the row ends, never its verdict.  The row state is the cost-only layout
+// (carve_cost_smem: cumulative transforms, world spheres, broad-phase bounds and masks), one persistent warp per row for every
+// robot; rows are handed out by the ticket counter.  a.cfg holds weight 1 and activation 0 for the scene and self terms.
+enum : int { kCheckBounds = 1, kCheckSelf = 2, kCheckScene = 4 };
+
+template <int SCENE>
+__device__ __forceinline__ bool validate_row(const FusedArgs &a, const RobotView &rv, const EvalSmem &es, int lane, int e, int b,
+                                             int checks) {
+  const int D = rv.D, S = rv.S;
+#pragma unroll 1
+  for (int d0 = 0; d0 < D; d0 += 32) {
+    const int d = d0 + lane;
+    bool out = false;
+    if (d < D) {
+      const float x = __ldg(a.q + (size_t)e * D + d);
+      es.qv[d] = x;
+      float c = 0.0f, g;
+      bound_cost(x, rv.limits[d], rv.limits[D + d], 0.0f, 1.0f, c, g);
+      out = (checks & kCheckBounds) && c != 0.0f;
+    }
+    if (__ballot_sync(kFull, out) != 0u) return false;
+  }
+  if (!(checks & (kCheckScene | kCheckSelf))) return true;
+  __syncwarp();
+  warp_fk<32>(rv, es, lane);
+  warp_spheres<32>(rv, es, lane, nullptr, row_sphere_cfg(a, b, S));
+  __syncwarp();
+  if (SCENE != 0 && (checks & kCheckScene)) {
+    const int env = a.env_query_idx != nullptr ? __ldg(a.env_query_idx + b) : 0;
+    CuboidCull cc{0, 0, false};
+    if (has_cuboids<SCENE>(a, true)) {
+      if (cuboid_cull_state(a, rv, env, true, cc)) {
+        cuboid_cull_masks(a, rv, es, cc.ce, cc.ncub, lane, 32);
+        __syncwarp();
+      }
+    }
+#pragma unroll 1
+    for (int s0 = 0; s0 < S; s0 += 32) {
+      const int s = s0 + lane;
+      V3 g = mk3(0, 0, 0);
+      const bool hit = s < S && sphere_discrete_terms<SCENE>(a, rv, es, cc, env, s, g) != 0.0f;
+      if (__ballot_sync(kFull, hit) != 0u) return false;
+    }
+  }
+  if ((checks & kCheckSelf) && rv.P > 0) {
+    int bi, bj;
+    const float f = rv.n_lp > 0 ? warp_self_collision_tiles<false, true, 32, true>(rv, es, lane, bi, bj)
+                                : warp_self_collision_pairs<32>(es.gsph, rv.pairs, rv.P, lane, bi, bj);
+    if (f > 0.0f) return false;
+  }
+  return true;
+}
+
+template <int SCENE>
+__global__ void __launch_bounds__(kWarpsPerCta * 32, kMinCtas) rollout_validate_kernel(const __grid_constant__ FusedArgs a,
+                                                                                       uint8_t *valid, const int checks) {
+  CB200_EXTERN_SHARED __align__(128) unsigned char smem[];
+  __shared__ unsigned long long mbar;
+  stage_blob_to_smem(smem, a.blob, (uint32_t)a.blob_smem_bytes, &mbar);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+  const bool leader = lane == 0;
+  float *base = reinterpret_cast<float *>(smem + a.blob_smem_bytes) + (size_t)warp * a.eval_floats;
+  const int N = a.B * a.H;
+  const int stride = gridDim.x * nwarps;
+  int e = blockIdx.x * nwarps + warp;
+  while (e < N) {
+    const int b = a.H != 1 ? e / a.H : e;
+    const RobotView rv = make_robot_view(smem, a.blob);
+    const EvalSmem es = carve_cost_smem(base, rv.nl, rv.D, rv.S, rv.n_cl, rv.n_lp == 0);
+    const bool ok = validate_row<SCENE>(a, rv, es, lane, e, b, checks);
+    if (leader) valid[e] = ok ? 1 : 0;
+    __syncwarp();  // the next row rewrites the row state
+    e = next_warp_unit(a.work_counter, e, stride, leader);
+  }
+  if (a.work_counter != nullptr && leader) rearm_ticket_counter(a.work_counter, stride);
+}
+
+// ------------------------------------------------------------------------------------------------
 // THE fused kernel for big robots (humanoids), discrete scene collision.  Same phases and arithmetic as rollout_fused_kernel;
 // what changes is how many rows an SM keeps in flight.  The kernel is latency bound and shared memory caps the resident warps: a G1-29 row is 17.3 KB, of which 12.8 KB
 // are two [S] float4 arrays -- the padded copy of the spheres for the pair phase and the dense sphere gradients.  Here
@@ -2915,6 +2997,66 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
 
 int cb200_rollout_cost(const cb200_rollout_cfg *cfg, const cb200_rollout_io *io, cb200_stream_t stream) {
   return rollout_launch(cfg, io, stream, false);
+}
+
+int cb200_rollout_validate(const cb200_rollout_io *io, uint8_t *valid, int32_t check_bounds, int32_t check_self,
+                           int32_t check_scene, cb200_stream_t stream) {
+  CB200_DEVICE_GUARD(valid);
+  if (io == nullptr || valid == nullptr || io->q == nullptr || io->robot_blob == nullptr || io->spline != nullptr ||
+      io->dynamics != nullptr || io->current_position != nullptr || io->batch_size < 0 || io->horizon < 1)
+    return ret(cudaErrorInvalidValue);
+  const long long N = (long long)io->batch_size * io->horizon;
+  if (N == 0) return ret(cudaSuccess);
+  if (io->robot_blob_host == nullptr || N > 0x7fffffffLL) return ret(cudaErrorInvalidValue);
+  BlobHeader h;
+  memcpy(&h, io->robot_blob_host, sizeof(BlobHeader));
+  if (h.magic != kBlobMagic || h.total_bytes != io->robot_blob_bytes) return ret(cudaErrorInvalidValue);
+  FusedArgs a{};
+  a.cfg.self_weight = 1.0f;
+  a.cfg.scene_weight = 1.0f;
+  a.cfg.scene_activation = 0.0f;
+  a.q = io->q;
+  a.blob = static_cast<const unsigned char *>(io->robot_blob);
+  a.env_query_idx = io->env_query_idx;
+  a.B = io->batch_size;
+  a.H = io->horizon;
+  a.blob_smem_bytes = h.smem_bytes;
+  a.eval_floats = cost_smem_floats(h.nl, h.D, h.S, h.n_cl, h.n_lp == 0);
+  if (io->sphere_configs != nullptr && io->num_sphere_configs > 1) {
+    if (h.n_sphere_cfgs != io->num_sphere_configs) return ret(cudaErrorInvalidValue);
+    a.sphere_cfgs = reinterpret_cast<const float4 *>(io->sphere_configs);
+    a.n_sphere_cfgs = io->num_sphere_configs;
+  }
+  int scene = 0;
+  if (check_scene) {
+    a.cuboids = to_dev(io->cuboids);
+    a.voxels = to_dev(io->voxels);
+    scene = (a.cuboids.inv_pose ? 1 : 0) | (a.voxels.inv_pose ? 2 : 0);
+    const cb200_mesh_set *m = io->meshes;
+    if (m != nullptr && m->inv_pose != nullptr) {
+      if (m->nodes == nullptr || m->triangles == nullptr || m->node_offset == nullptr || m->triangle_offset == nullptr ||
+          m->dims == nullptr || m->enable == nullptr || m->count == nullptr)
+        return ret(cudaErrorInvalidValue);
+      a.meshes = MeshSet{reinterpret_cast<const float4 *>(m->nodes), reinterpret_cast<const float4 *>(m->triangles), m->node_offset,
+                         m->triangle_offset, m->dims, m->inv_pose, m->enable, m->count, m->max_n, m->num_envs};
+      scene = 7;
+    }
+  }
+  const void *kernel = by_scene<true>(scene, [](auto c) { return rollout_validate_kernel<c>; });
+  const DevInfo &d = dev_info();
+  Plan p;
+  const PlanKey key{kernel, d.ordinal, (size_t)h.smem_bytes, a.eval_floats, 0, 0, 0};
+  if (const cudaError_t e = cached_plan(key, d, [](const PlanKey &k, size_t limit) { return plan_warps(k, limit, kWarpsPerCta); }, p);
+      e != cudaSuccess)
+    return ret(e);
+  if (p.nw == 0) return ret(cudaErrorInvalidConfiguration);
+  const long long resident = (long long)d.sm_count * p.per_sm, need = (N + p.nw - 1) / p.nw;
+  if (need > resident) a.work_counter = env_int("CB200_QUEUE", 1) != 0 ? io->work_counter : nullptr;
+  const int checks = (check_bounds ? kCheckBounds : 0) | (check_self ? kCheckSelf : 0) | (check_scene ? kCheckScene : 0);
+  g_last_variant = CB200_VARIANT_VALIDATE;
+  CB200_LAUNCH(((void (*)(const FusedArgs, uint8_t *, const int))kernel), (int)std::max(std::min(resident, need), 1LL), p.nw * 32,
+               p.smem, (cudaStream_t)stream, a, valid, checks);
+  return launch_status();
 }
 
 }  // extern "C"

@@ -428,7 +428,9 @@ __device__ __forceinline__ float4 padded_sphere(const RobotView &rv, const EvalS
 // key_out: the warp's reduced arg-max key (f bits | ~i | ~j), 0 when nothing is positive.
 // CULL2 = false (arm build of the IK kernel: links of <= ~10 spheres): blocks are scanned whole -- the second-level cull's code is
 // 1.6 KB of the row's instruction footprint, which is what that kernel is short of.
-template <bool PADDED_COPY = true, bool CULL2 = true, int W = 32>
+// ANY = true (validity rows): the row only asks whether some pair has f > 0, so the scan stops at the first block boundary where
+// a lane holds one (a warp vote); the returned f and pair are then those of the blocks scanned so far.
+template <bool PADDED_COPY = true, bool CULL2 = true, int W = 32, bool ANY = false>
 __device__ __forceinline__ float warp_self_collision_tiles(const RobotView &rv, const EvalSmem &es, int lane, int &bi,
                                                            int &bj, int base0 = 0, int stride = W,
                                                            unsigned char *idx_scratch = nullptr,
@@ -451,6 +453,7 @@ __device__ __forceinline__ float warp_self_collision_tiles(const RobotView &rv, 
     }
     unsigned m = row_ballot<W>(hit);
     while (m) {
+      if (ANY && row_ballot<W>(key != 0ull) != 0u) break;
       const int src = __ffs(m) - 1;
       m &= m - 1;
       const uint32_t q = row_shfl<W>(pr, src);
@@ -517,6 +520,7 @@ __device__ __forceinline__ float warp_self_collision_tiles(const RobotView &rv, 
         }
       }
     }
+    if (ANY && row_ballot<W>(key != 0ull) != 0u) break;
   }
 #pragma unroll
   for (int o = W / 2; o > 0; o >>= 1) {

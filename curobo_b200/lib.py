@@ -122,9 +122,11 @@ _SIGS = {
     "cb200_refresh_robot_spheres": ([c_p, c_p, C.c_int32, c_p, C.c_int32, c_p], _I),
     "cb200_rollout_cost_grad": ([C.POINTER(RolloutCfg), C.POINTER(RolloutIO), c_p], _I),
     "cb200_rollout_cost": ([C.POINTER(RolloutCfg), C.POINTER(RolloutIO), c_p], _I),
+    "cb200_rollout_validate": ([C.POINTER(RolloutIO), c_p, C.c_int32, C.c_int32, C.c_int32, c_p], _I),
 }
 
 VARIANT_COST_ONLY = 0x10    # include/curobo_b200.h: CB200_VARIANT_COST_ONLY, or'd into cb200_last_rollout_variant()
+VARIANT_VALIDATE = 0x20     # include/curobo_b200.h: CB200_VARIANT_VALIDATE
 
 EXPORTED_SYMBOLS = tuple(_SIGS.keys())
 

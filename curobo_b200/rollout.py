@@ -640,9 +640,32 @@ class RolloutEngine:
             use_implicit_goal_state, B, H, D)
         return out
 
-    def _launch(self, io, B: int, H: int, env_query_idx, grad: bool = True, with_terms: bool = True) -> RolloutOutput:
+    def validate(self, q: torch.Tensor, env_query_idx: Optional[torch.Tensor] = None, check_bounds: bool = True,
+                 check_self: bool = True, check_scene: bool = True) -> torch.Tensor:
+        """Validity of joint configurations q [B, H, D] -> torch.bool [B, H] (cb200_rollout_validate; the reference's
+        RobotSceneCollision.validate): a row is valid iff it is inside the position limits (check_bounds), no pair of the
+        self-collision pair list overlaps with padded radii (check_self), and no enabled sphere touches an enabled obstacle of
+        the row's environment, r - sdf > 0 (check_scene).  Independent of `cfg`: the terms are tested at activation 0.  H > 1
+        rows are independent discrete rows.  The output buffer is allocated once per (B, H) and returned as a bool view of it,
+        so the call is CUDA-graph capturable; a later call with the same (B, H) overwrites it."""
+        if q.ndim != 3 or q.shape[2] != self.robot.num_dof:
+            raise ValueError(f"q must be [B, H, {self.robot.num_dof}], got {tuple(q.shape)}")
+        check_tensors(self.device, torch.float32, q=q)
+        B, H, _ = q.shape
+        if getattr(self, "_valid", None) is None or tuple(self._valid.shape) != (B, H):
+            self._valid = torch.zeros((B, H), dtype=torch.uint8, device=self.device)
+        io = _lib.RolloutIO()
+        io.q = q.data_ptr()
+        io.batch_size, io.horizon = B, H
+        self._world_io(io, env_query_idx)
+        err = self._lib.cb200_rollout_validate(C.byref(io), self._valid.data_ptr(), int(bool(check_bounds)), int(bool(check_self)),
+                                               int(bool(check_scene)), stream_ptr(self.device))
+        _lib.check(err, "rollout_validate")
+        return self._valid.view(torch.bool)
+
+    def _world_io(self, io, env_query_idx) -> None:
+        """The robot blob, the obstacle sets, env_query_idx, the sphere configurations and the ticket counter into io."""
         dev = self.device
-        o = self.out
         io.robot_blob, io.robot_blob_host = self._blob.data_ptr(), self._blob_host.ctypes.data
         io.robot_blob_bytes = int(self._blob_host.shape[0])
         if self._cs is not None:
@@ -661,6 +684,18 @@ class RolloutEngine:
         if env_query_idx is not None:
             check_tensors(dev, torch.int32, env_query_idx=env_query_idx)
             io.env_query_idx = env_query_idx.data_ptr()
+        if self.link_spheres._version != self._link_spheres_version:   # written in place since the last refresh
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("link_spheres changed since the last refresh; call refresh_link_spheres() before capturing")
+            self.refresh_link_spheres()
+        if self.link_spheres.shape[0] > 1:
+            io.sphere_configs, io.num_sphere_configs = self.link_spheres.data_ptr(), int(self.link_spheres.shape[0])
+        io.work_counter = self._work_counter.data_ptr()
+
+    def _launch(self, io, B: int, H: int, env_query_idx, grad: bool = True, with_terms: bool = True) -> RolloutOutput:
+        dev = self.device
+        o = self.out
+        self._world_io(io, env_query_idx)
         if self._goal is not None and self.cfg.pose_weight is not None:
             gp, gq, ig, extra = self._goal
             if ig.shape[0] != B:
@@ -690,12 +725,6 @@ class RolloutEngine:
                 io.current_velocity = cv.data_ptr()
             if cidx is not None:
                 io.idxs_current_state = cidx.data_ptr()
-        if self.link_spheres._version != self._link_spheres_version:   # written in place since the last refresh
-            if torch.cuda.is_current_stream_capturing():
-                raise RuntimeError("link_spheres changed since the last refresh; call refresh_link_spheres() before capturing")
-            self.refresh_link_spheres()
-        if self.link_spheres.shape[0] > 1:
-            io.sphere_configs, io.num_sphere_configs = self.link_spheres.data_ptr(), int(self.link_spheres.shape[0])
         io.cost = o.cost.data_ptr()
         if grad:
             io.grad_q = o.grad_q.data_ptr()
@@ -709,7 +738,6 @@ class RolloutEngine:
             if t is not None:
                 setattr(io, name, t.data_ptr())
         io.batch_size, io.horizon = B, H
-        io.work_counter = self._work_counter.data_ptr()
         if self._dyn_params is not None and io.vel and io.acc and not bool(io.spline):
             io.dynamics = C.pointer(self._dyn_params)
         if self._ms is not None and self.cfg.scene_weight > 0.0:

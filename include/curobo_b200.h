@@ -46,6 +46,7 @@ const char *cb200_error_string(int err);
 #define CB200_VARIANT_TRAJ 7     /* rollout_traj_kernel: trajectory mode (swept collision, state costs) */
 #define CB200_VARIANT_TRAJ_DYN 8 /* rollout_traj_dyn_kernel: trajectory mode + inverse dynamics */
 #define CB200_VARIANT_COST_ONLY 0x10 /* bit: cb200_rollout_cost (rollout_cost_kernel / rollout_cost_big_kernel) */
+#define CB200_VARIANT_VALIDATE 0x20  /* bit: cb200_rollout_validate (rollout_validate_kernel) */
 int cb200_last_rollout_variant(void);
 
 /* -------------------------------------------------------------------------------------------
@@ -381,6 +382,22 @@ int cb200_rollout_cost_grad(const cb200_rollout_cfg *cfg, const cb200_rollout_io
  * Covers discrete rows from io->q: use_sweep, a spline front end or dynamics return cudaErrorInvalidValue, as do a NULL
  * cost, robot_blob or q.  cb200_last_rollout_variant() reports the variant of the kernel it twins | CB200_VARIANT_COST_ONLY. */
 int cb200_rollout_cost(const cb200_rollout_cfg *cfg, const cb200_rollout_io *io, cb200_stream_t stream);
+
+/* Validity of joint configurations (the reference's RobotSceneCollision.validate, collision_robot_scene.py:341-372): valid[b,h] = 1
+ * iff every check asked for holds, else 0.
+ *   check_bounds: position limits of the blob, lower[d] <= q[d] <= upper[d] (the POSITION c-space bound cost at weight 1 and
+ *                 activation 0 is exactly 0);
+ *   check_self:   no pair of the self-collision pair list with both padded radii >= 0 overlaps, (r_i + r_j)^2 - |p_i - p_j|^2 > 0;
+ *   check_scene:  no sphere with r >= 0 touches an enabled obstacle of the row's environment, r - sdf > 0 (cuboids, ESDF grids
+ *                 and meshes with the SDF arithmetic of the fused kernels; env_query_idx and sphere_configs apply as there).
+ * H > 1 rows are independent discrete rows (no sweep).  One persistent warp per row; a row stops at its first failed check
+ * (bounds before FK, then scene, then self), which changes the time it takes, never its verdict.
+ * Reads only q, robot_blob, robot_blob_host, robot_blob_bytes, cuboids, voxels, meshes, env_query_idx, sphere_configs,
+ * num_sphere_configs, work_counter, batch_size and horizon; every cost and gradient field is ignored.  Returns
+ * cudaErrorInvalidValue for a NULL valid, io, q or robot_blob, and when spline, dynamics or current_position is set.
+ * cb200_last_rollout_variant() reports CB200_VARIANT_VALIDATE.  Allocates nothing and never synchronises (graph-capturable). */
+int cb200_rollout_validate(const cb200_rollout_io *io, uint8_t *valid /* [B,H] */, int32_t check_bounds, int32_t check_self,
+                           int32_t check_scene, cb200_stream_t stream);
 
 /* -------------------------------------------------------------------------------------------
  * (8f-1) B-spline knot -> state kernels and their adjoint: the step in front of / behind the rollout
