@@ -11,17 +11,19 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "../../include/curobo_b200.h"
 #include "cb200_launch.h"
 #include "cb200_dynamics.cuh"
 
 namespace {
 using namespace cb200::dyn;
-
-inline int status(cudaError_t e) {
-  if (e != cudaSuccess) (void)cudaGetLastError();
-  return (int)e;
-}
+using cb200::capped_grid;
+using cb200::dev_info;
+using cb200::launch_status;
+using cb200::opt_in_smem;
+using cb200::ret;
 
 struct TileStore {  // [arr][link][comp][rows] floats in shared memory
   float *base;
@@ -410,11 +412,8 @@ struct CtaPlan {
 };
 // rows per CTA: the largest of 32 / 16 / 8 that keeps two CTAs per SM resident, halved while the grid would leave SMs idle
 CtaPlan plan_cta(int B, int floats_per_row, int model_floats, bool adjoint) {
-  int dev = 0, max_smem = 227 * 1024, sms = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) {
-    cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  }
+  const cb200::DevInfo &d = dev_info();
+  const int max_smem = d.max_smem, sms = d.sm_count;
   CtaPlan p;
   auto bytes = [&](int R) { return (floats_per_row * (R + 1) + model_floats) * (int)sizeof(float); };
   // tuning (scripts/bench_dynamics.py, not repeated on H100): the adjoint is fastest at 16 rows per CTA, the forward pass at 32 once
@@ -430,46 +429,25 @@ CtaPlan plan_cta(int B, int floats_per_row, int model_floats, bool adjoint) {
   if (bytes(R) > max_smem) return p;
   p.R = R;
   p.smem = bytes(R);
-  long long gsz = ((long long)B + R - 1) / R;
-  if (gsz > (long long)sms * 32) gsz = (long long)sms * 32;
-  p.grid = (int)gsz;
+  p.grid = capped_grid(((long long)B + R - 1) / R, 32);
   return p;
-}
-template <class K>
-bool allow_smem(K kern, int smem) {
-  if (smem <= 48 * 1024) return true;
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess) return true;
-  (void)cudaGetLastError();
-  return false;
 }
 inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // rows per CTA: the largest of 128 / 64 / 32 whose tile leaves room for two CTAs per SM, else the largest of 32 .. 4 that fits
 template <class K>
 int pick_rows(K kern, int floats_per_row, int &smem_out) {
-  int dev = 0, max_smem = 227 * 1024;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  const int max_smem = dev_info().max_smem;
   for (int rows = 128; rows >= 4; rows >>= 1) {  // below a warp for very large trees: correctness first on this path
     const int smem = floats_per_row * rows * (int)sizeof(float);
     if (smem * 2 + 4096 <= max_smem || (rows <= 32 && smem <= max_smem) || rows == 4) {
       if (smem > max_smem) return 0;
-      if (smem > 48 * 1024 && cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
-        (void)cudaGetLastError();
-        continue;
-      }
+      if (opt_in_smem(kern, smem) != cudaSuccess) continue;
       smem_out = smem;
       return rows;
     }
   }
   return 0;
-}
-
-int grid_for(int B, int rows) {
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  long long g = ((long long)B + rows - 1) / rows;
-  if (g > (long long)sms * 8) g = (long long)sms * 8;
-  return (int)(g < 1 ? 1 : g);
 }
 
 bool model_ok(const Model &M) {
@@ -490,28 +468,25 @@ int cb200_rnea_forward(float *tau, const float *q, const float *qd, const float 
           level_starts,     level_links,     num_links,     num_dof,        n_levels};
   if (!model_ok(M) || tau == nullptr || q == nullptr || qd == nullptr || qdd == nullptr || forward_cache == nullptr ||
       batch_size < 0)
-    return status(cudaErrorInvalidValue);
-  if (batch_size == 0) return status(cudaSuccess);
+    return ret(cudaErrorInvalidValue);
+  if (batch_size == 0) return ret(cudaSuccess);
   FwdArgs a{M, tau, forward_cache, q, qd, qdd, f_ext, batch_size};
   const CtaPlan p = plan_cta(batch_size, (2 * 6 + 2) * num_links + 4 * num_dof, model_smem_floats_host(num_links, n_levels), false);
   if (p.R != 0 && aligned16(forward_cache) && getenv("CB200_RNEA_ROWS") == nullptr) {
-    const cudaStream_t st = (cudaStream_t)stream;
-    if (p.R == 32 && allow_smem(rnea_forward_cta<32>, p.smem)) {
-      CB200_LAUNCH(rnea_forward_cta<32>, p.grid, kThreads, p.smem, st, a);
-      return status(cudaGetLastError());
-    } else if (p.R == 16 && allow_smem(rnea_forward_cta<16>, p.smem)) {
-      CB200_LAUNCH(rnea_forward_cta<16>, p.grid, kThreads, p.smem, st, a);
-      return status(cudaGetLastError());
-    } else if (p.R == 8 && allow_smem(rnea_forward_cta<8>, p.smem)) {
-      CB200_LAUNCH(rnea_forward_cta<8>, p.grid, kThreads, p.smem, st, a);
-      return status(cudaGetLastError());
-    }
+    auto cta = [&](auto R) {  // false: the shared-memory opt-in failed, the rows kernel below runs instead
+      if (opt_in_smem(rnea_forward_cta<R>, p.smem) != cudaSuccess) return false;
+      CB200_LAUNCH(rnea_forward_cta<R>, p.grid, kThreads, p.smem, (cudaStream_t)stream, a);
+      return true;
+    };
+    if ((p.R == 32 && cta(std::integral_constant<int, 32>{})) || (p.R == 16 && cta(std::integral_constant<int, 16>{})) ||
+        (p.R == 8 && cta(std::integral_constant<int, 8>{})))
+      return launch_status();
   }
   int smem = 0;  // very large trees: one thread per row over a two-array tile
   const int rows = pick_rows(rnea_forward_rows, 2 * num_links * 6, smem);
-  if (rows == 0) return status(cudaErrorInvalidConfiguration);
-  CB200_LAUNCH(rnea_forward_rows, grid_for(batch_size, rows), rows, smem, (cudaStream_t)stream, a);
-  return status(cudaGetLastError());
+  if (rows == 0) return ret(cudaErrorInvalidConfiguration);
+  CB200_LAUNCH(rnea_forward_rows, capped_grid(((long long)batch_size + rows - 1) / rows, 8), rows, smem, (cudaStream_t)stream, a);
+  return launch_status();
 }
 
 int cb200_rnea_backward(float *grad_q, float *grad_qd, float *grad_qdd, const float *grad_tau, const float *q,
@@ -525,28 +500,25 @@ int cb200_rnea_backward(float *grad_q, float *grad_qd, float *grad_qdd, const fl
           level_starts,     level_links,     num_links,     num_dof,        n_levels};
   if (!model_ok(M) || grad_q == nullptr || grad_qd == nullptr || grad_qdd == nullptr || grad_tau == nullptr || q == nullptr ||
       qd == nullptr || forward_cache == nullptr || batch_size < 0)
-    return status(cudaErrorInvalidValue);
-  if (batch_size == 0) return status(cudaSuccess);
+    return ret(cudaErrorInvalidValue);
+  if (batch_size == 0) return ret(cudaSuccess);
   BwdArgs a{M, grad_q, grad_qd, grad_qdd, grad_f_ext, grad_tau, q, qd, forward_cache, batch_size};
   const CtaPlan p = plan_cta(batch_size, (5 * 6 + 2) * num_links + 6 * num_dof, 0, true);
   if (p.R != 0 && aligned16(forward_cache) && getenv("CB200_RNEA_ROWS") == nullptr) {
-    const cudaStream_t st = (cudaStream_t)stream;
-    if (p.R == 32 && allow_smem(rnea_backward_cta<32>, p.smem)) {
-      CB200_LAUNCH(rnea_backward_cta<32>, p.grid, kThreads, p.smem, st, a);
-      return status(cudaGetLastError());
-    } else if (p.R == 16 && allow_smem(rnea_backward_cta<16>, p.smem)) {
-      CB200_LAUNCH(rnea_backward_cta<16>, p.grid, kThreads, p.smem, st, a);
-      return status(cudaGetLastError());
-    } else if (p.R == 8 && allow_smem(rnea_backward_cta<8>, p.smem)) {
-      CB200_LAUNCH(rnea_backward_cta<8>, p.grid, kThreads, p.smem, st, a);
-      return status(cudaGetLastError());
-    }
+    auto cta = [&](auto R) {
+      if (opt_in_smem(rnea_backward_cta<R>, p.smem) != cudaSuccess) return false;
+      CB200_LAUNCH(rnea_backward_cta<R>, p.grid, kThreads, p.smem, (cudaStream_t)stream, a);
+      return true;
+    };
+    if ((p.R == 32 && cta(std::integral_constant<int, 32>{})) || (p.R == 16 && cta(std::integral_constant<int, 16>{})) ||
+        (p.R == 8 && cta(std::integral_constant<int, 8>{})))
+      return launch_status();
   }
   int smem = 0;
   const int rows = pick_rows(rnea_backward_rows, 5 * num_links * 6, smem);
-  if (rows == 0) return status(cudaErrorInvalidConfiguration);
-  CB200_LAUNCH(rnea_backward_rows, grid_for(batch_size, rows), rows, smem, (cudaStream_t)stream, a);
-  return status(cudaGetLastError());
+  if (rows == 0) return ret(cudaErrorInvalidConfiguration);
+  CB200_LAUNCH(rnea_backward_rows, capped_grid(((long long)batch_size + rows - 1) / rows, 8), rows, smem, (cudaStream_t)stream, a);
+  return launch_status();
 }
 
 }  // extern "C"

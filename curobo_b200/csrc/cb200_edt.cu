@@ -23,11 +23,10 @@
 
 namespace {
 using namespace cb200::edt;
-
-inline int status(cudaError_t e) {
-  if (e != cudaSuccess) (void)cudaGetLastError();
-  return (int)e;
-}
+using cb200::capped_grid;
+using cb200::launch_status;
+using cb200::opt_in_smem;
+using cb200::ret;
 
 // pass 1.  A warp per z-row; CHUNKS x 32 >= nz.  v[c] = the row's voxels c * 32 + lane.  Forward: the last site at or
 // before a voxel = highest set bit of the chunk's site ballot at or below the lane (else the carry of the earlier chunks);
@@ -302,19 +301,6 @@ __global__ void __launch_bounds__(256) tsdf_stamp_cuboids_kernel(float *__restri
   }
 }
 
-template <class K>
-bool allow_smem(K kern, int smem) {
-  if (smem <= 48 * 1024) return true;
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess) return true;
-  (void)cudaGetLastError();
-  return false;
-}
-int grid_for(long long tiles) {
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const long long cap = (long long)sms * 32;
-  return (int)(tiles < 1 ? 1 : (tiles > cap ? cap : tiles));
-}
 bool dims_ok(int nx, int ny, int nz) {
   return nx >= 1 && ny >= 1 && nz >= 1 && nx <= kMaxDim && ny <= kMaxDim && nz <= kMaxDim &&
          (long long)nx * ny * nz <= 2147483647LL;
@@ -327,16 +313,16 @@ int cb200_pba3d(int32_t *site_index, int32_t *buffer, int nx, int ny, int nz, in
   CB200_DEVICE_GUARD(site_index);
   (void)buffer;  // the reference's ping-pong scratch: every pass here is in place
   (void)m3;      // the reference's colour-kernel block height
-  if (site_index == nullptr || !dims_ok(nx, ny, nz)) return status(cudaErrorInvalidValue);
+  if (site_index == nullptr || !dims_ok(nx, ny, nz)) return ret(cudaErrorInvalidValue);
   const cudaStream_t st = (cudaStream_t)stream;
   const Plan p = make_plan(site_index, nx, ny, nz);
   const BandedEnvelope<1> by{p.y};
   const BandedEnvelope<0> bx{p.x};
   const int smem_y = by.smem_ints() * (int)sizeof(int), smem_x = bx.smem_ints() * (int)sizeof(int);
-  if (!allow_smem(edt_envelope_kernel<1>, smem_y) || !allow_smem(edt_envelope_kernel<0>, smem_x))
-    return status(cudaErrorInvalidConfiguration);
+  if (opt_in_smem(edt_envelope_kernel<1>, smem_y) != cudaSuccess || opt_in_smem(edt_envelope_kernel<0>, smem_x) != cudaSuccess)
+    return ret(cudaErrorInvalidConfiguration);
   const long long nrows = (long long)nx * ny;
-  const int zgrid = grid_for((nrows + 15) / 16);  // 8 warps per CTA, two rows per warp and step
+  const int zgrid = capped_grid((nrows + 15) / 16, 32);  // 8 warps per CTA, two rows per warp and step
   if (nz <= 128) {
     CB200_LAUNCH(edt_flood_z_kernel<4>, zgrid, 256, 0, st, site_index, nz, nrows);
   } else if (nz <= 256) {
@@ -346,43 +332,43 @@ int cb200_pba3d(int32_t *site_index, int32_t *buffer, int nx, int ny, int nz, in
   } else {
     CB200_LAUNCH(edt_flood_z_kernel<32>, zgrid, 256, 0, st, site_index, nz, nrows);
   }
-  CB200_LAUNCH(edt_envelope_kernel<1>, grid_for(by.e.ntiles()), kBands * kLanes, smem_y, st, by);
-  CB200_LAUNCH(edt_envelope_kernel<0>, grid_for(bx.e.ntiles()), kBands * kLanes, smem_x, st, bx);
-  return status(cudaGetLastError());
+  CB200_LAUNCH(edt_envelope_kernel<1>, capped_grid(by.e.ntiles(), 32), kBands * kLanes, smem_y, st, by);
+  CB200_LAUNCH(edt_envelope_kernel<0>, capped_grid(bx.e.ntiles(), 32), kBands * kLanes, smem_x, st, bx);
+  return launch_status();
 }
 
 int cb200_edt_unsigned_distance(const int32_t *site_index, uint16_t *distance_fp16, int nx, int ny, int nz, float voxel_size,
                                 float empty_value, cb200_stream_t stream) {
   CB200_DEVICE_GUARD(distance_fp16);
   if (site_index == nullptr || distance_fp16 == nullptr || !dims_ok(nx, ny, nz) || !(voxel_size > 0.0f))
-    return status(cudaErrorInvalidValue);
+    return ret(cudaErrorInvalidValue);
   const long long total = (long long)nx * ny * nz;
   const long long blocks = (total + 255) / 256;
-  CB200_LAUNCH(edt_distance_kernel, grid_for(blocks), 256, 0, (cudaStream_t)stream, site_index, reinterpret_cast<__half *>(distance_fp16),
+  CB200_LAUNCH(edt_distance_kernel, capped_grid(blocks, 32), 256, 0, (cudaStream_t)stream, site_index, reinterpret_cast<__half *>(distance_fp16),
                ny, nz, total, voxel_size, empty_value);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 int cb200_esdf_seed_sites(const float *combined_sdf, int32_t *site_index, int nx, int ny, int nz, float voxel_size,
                           float truncation_distance, cb200_stream_t stream) {
   CB200_DEVICE_GUARD(site_index);
   if (combined_sdf == nullptr || site_index == nullptr || !dims_ok(nx, ny, nz) || !(voxel_size > 0.0f))
-    return status(cudaErrorInvalidValue);
+    return ret(cudaErrorInvalidValue);
   const long long total = (long long)nx * ny * nz;
-  CB200_LAUNCH(esdf_seed_sites_kernel, grid_for((total + 255) / 256), 256, 0, (cudaStream_t)stream, combined_sdf, site_index, ny, nz,
+  CB200_LAUNCH(esdf_seed_sites_kernel, capped_grid((total + 255) / 256, 32), 256, 0, (cudaStream_t)stream, combined_sdf, site_index, ny, nz,
                total, voxel_size, truncation_distance);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 int cb200_esdf_seed_sites_gather(const float *combined_sdf, int32_t *site_index, int nx, int ny, int nz, float voxel_size,
                                  float truncation_distance, const float *origin, cb200_stream_t stream) {
   CB200_DEVICE_GUARD(site_index);
   if (combined_sdf == nullptr || site_index == nullptr || origin == nullptr || !dims_ok(nx, ny, nz) || !(voxel_size > 0.0f))
-    return status(cudaErrorInvalidValue);
+    return ret(cudaErrorInvalidValue);
   const long long total = (long long)nx * ny * nz;
-  CB200_LAUNCH(esdf_seed_sites_gather_kernel, grid_for((total + 255) / 256), 256, 0, (cudaStream_t)stream, combined_sdf, site_index, nx,
+  CB200_LAUNCH(esdf_seed_sites_gather_kernel, capped_grid((total + 255) / 256, 32), 256, 0, (cudaStream_t)stream, combined_sdf, site_index, nx,
                ny, nz, total, voxel_size, truncation_distance, origin[0], origin[1], origin[2]);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 int cb200_esdf_signed_distance(const int32_t *site_index, const float *static_sdf, const float *combined_sdf,
@@ -390,11 +376,11 @@ int cb200_esdf_signed_distance(const int32_t *site_index, const float *static_sd
                                cb200_stream_t stream) {
   CB200_DEVICE_GUARD(distance_fp16);
   if (site_index == nullptr || distance_fp16 == nullptr || !dims_ok(nx, ny, nz) || !(voxel_size > 0.0f))
-    return status(cudaErrorInvalidValue);
+    return ret(cudaErrorInvalidValue);
   const long long total = (long long)nx * ny * nz;
-  CB200_LAUNCH(esdf_signed_distance_kernel, grid_for((total + 255) / 256), 256, 0, (cudaStream_t)stream, site_index, static_sdf,
+  CB200_LAUNCH(esdf_signed_distance_kernel, capped_grid((total + 255) / 256, 32), 256, 0, (cudaStream_t)stream, site_index, static_sdf,
                combined_sdf, reinterpret_cast<__half *>(distance_fp16), nx, ny, nz, total, voxel_size, adjacent_skip_steps);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 int cb200_tsdf_integrate_depth(uint16_t *block_data_fp16, int nx, int ny, int nz, float voxel_size, const float *origin,
@@ -405,13 +391,13 @@ int cb200_tsdf_integrate_depth(uint16_t *block_data_fp16, int nx, int ny, int nz
   if (block_data_fp16 == nullptr || origin == nullptr || intrinsics == nullptr || cam_positions == nullptr ||
       cam_quaternions == nullptr || depth_images == nullptr || !dims_ok(nx, ny, nz) || !(voxel_size > 0.0f) || num_cameras < 1 ||
       image_height < 1 || image_width < 1 || !(truncation_distance > 0.0f))
-    return status(cudaErrorInvalidValue);
+    return ret(cudaErrorInvalidValue);
   const long long total = (long long)nx * ny * nz;
   const TsdfCameras cams{intrinsics, cam_positions, cam_quaternions, depth_images, num_cameras, image_height, image_width};
-  CB200_LAUNCH(tsdf_integrate_depth_kernel, grid_for((total + 255) / 256), 256, 0, (cudaStream_t)stream,
+  CB200_LAUNCH(tsdf_integrate_depth_kernel, capped_grid((total + 255) / 256, 32), 256, 0, (cudaStream_t)stream,
                reinterpret_cast<__half *>(block_data_fp16), nx, ny, nz, total, voxel_size, origin[0], origin[1], origin[2], cams,
                depth_min, depth_max, truncation_distance);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 int cb200_tsdf_stamp_cuboids(float *static_sdf, int nx, int ny, int nz, float voxel_size, const float *origin,
@@ -420,21 +406,21 @@ int cb200_tsdf_stamp_cuboids(float *static_sdf, int nx, int ny, int nz, float vo
   if (static_sdf == nullptr || origin == nullptr || cuboids == nullptr || cuboids->inv_pose == nullptr || cuboids->dims == nullptr ||
       cuboids->enable == nullptr || cuboids->count == nullptr || cuboids->max_n < 1 || env_idx < 0 || env_idx >= cuboids->num_envs ||
       !dims_ok(nx, ny, nz) || !(voxel_size > 0.0f) || !(truncation_distance > 0.0f))
-    return status(cudaErrorInvalidValue);
+    return ret(cudaErrorInvalidValue);
   const long long total = (long long)nx * ny * nz;
   const cb200::CuboidSet cs{cuboids->dims, cuboids->inv_pose, cuboids->enable, cuboids->count, cuboids->max_n, cuboids->num_envs};
-  CB200_LAUNCH(tsdf_stamp_cuboids_kernel, grid_for((total + 255) / 256), 256, 0, (cudaStream_t)stream, static_sdf, nx, ny, nz, total,
+  CB200_LAUNCH(tsdf_stamp_cuboids_kernel, capped_grid((total + 255) / 256, 32), 256, 0, (cudaStream_t)stream, static_sdf, nx, ny, nz, total,
                voxel_size, origin[0], origin[1], origin[2], truncation_distance, cs, env_idx);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 int cb200_tsdf_combined_sdf(const uint16_t *block_data_fp16, const float *static_sdf, float *combined_sdf, long long num_voxels,
                             float min_weight, cb200_stream_t stream) {
   CB200_DEVICE_GUARD(combined_sdf);
-  if (block_data_fp16 == nullptr || combined_sdf == nullptr || num_voxels < 1) return status(cudaErrorInvalidValue);
-  CB200_LAUNCH(tsdf_combined_sdf_kernel, grid_for((num_voxels + 255) / 256), 256, 0, (cudaStream_t)stream,
+  if (block_data_fp16 == nullptr || combined_sdf == nullptr || num_voxels < 1) return ret(cudaErrorInvalidValue);
+  CB200_LAUNCH(tsdf_combined_sdf_kernel, capped_grid((num_voxels + 255) / 256, 32), 256, 0, (cudaStream_t)stream,
                reinterpret_cast<const __half *>(block_data_fp16), static_sdf, combined_sdf, num_voxels, min_weight);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 }  // extern "C"

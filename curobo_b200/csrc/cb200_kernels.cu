@@ -1907,45 +1907,6 @@ __global__ void __launch_bounds__(128) cspace_position_kernel(const __grid_const
 // ------------------------------------------------------------------------------------------------
 // host helpers
 // ------------------------------------------------------------------------------------------------
-inline int ret(cudaError_t e) {
-  if (e != cudaSuccess) (void)cudaGetLastError();  // do not leave a stale error for the caller's next CUDA call
-  return (int)e;
-}
-inline int launch_status() { return ret(cudaGetLastError()); }
-
-// Properties of the CURRENT device (the host layer makes the tensors' device current around every call), cached per
-// ordinal: one process may drive several GPUs, and cudaFuncSetAttribute / occupancy results are per device.
-struct DevInfo {
-  int sm_count = 0, max_smem = 0, ordinal = 0;
-  bool ok = false;
-};
-constexpr int kMaxDevices = 64;
-DevInfo &dev_info() {
-  static thread_local DevInfo table[kMaxDevices];
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) dev = 0;
-  DevInfo &d = table[dev];
-  if (!d.ok) {
-    d.ordinal = dev;
-    cudaDeviceGetAttribute(&d.sm_count, cudaDevAttrMultiProcessorCount, dev);
-    cudaDeviceGetAttribute(&d.max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    d.ok = d.sm_count > 0;
-  }
-  return d;
-}
-
-template <typename K>
-int persistent_grid(K kernel, int block, size_t smem, long long work_items) {
-  DevInfo &d = dev_info();
-  int per_sm = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, smem);
-  if (per_sm < 1) per_sm = 1;
-  long long g = (long long)d.sm_count * per_sm;
-  if (g > work_items) g = work_items;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-
 // Launch plan of a fused rollout kernel: its CTA shape for one robot geometry on one device.  The key holds everything the plan
 // depends on and is compared field by field.
 struct PlanKey {
@@ -2077,6 +2038,33 @@ inline VoxelSet to_dev(const cb200_voxel_set *v) {
                  v->max_n,  v->num_envs, v->max_dist, v->mip, v->mip_stride};
   return o;
 }
+// No meshes (o empty) when there is no set or it has no poses; a set with poses must give every array the kernels read.
+inline cudaError_t to_dev(const cb200_mesh_set *m, MeshSet &o) {
+  o = {};
+  if (m == nullptr || m->inv_pose == nullptr) return cudaSuccess;
+  if (m->nodes == nullptr || m->triangles == nullptr || m->node_offset == nullptr || m->triangle_offset == nullptr ||
+      m->dims == nullptr || m->enable == nullptr || m->count == nullptr)
+    return cudaErrorInvalidValue;
+  o = MeshSet{reinterpret_cast<const float4 *>(m->nodes), reinterpret_cast<const float4 *>(m->triangles), m->node_offset,
+              m->triangle_offset, m->dims, m->inv_pose, m->enable, m->count, m->max_n, m->num_envs};
+  return cudaSuccess;
+}
+
+// The header of the robot blob from its host copy; false unless that copy is a packed blob of exactly `bytes` bytes.
+bool read_blob_header(const void *host, int32_t bytes, BlobHeader &h) {
+  if (host == nullptr || bytes < (int32_t)sizeof(BlobHeader)) return false;
+  memcpy(&h, host, sizeof(BlobHeader));
+  return h.magic == kBlobMagic && h.total_bytes == bytes;
+}
+
+// Per-environment sphere configurations, when the caller gives more than one: the blob's broad-phase bounds must cover them all.
+cudaError_t set_sphere_cfgs(const cb200_rollout_io *io, const BlobHeader &h, FusedArgs &a) {
+  if (io->sphere_configs == nullptr || io->num_sphere_configs <= 1) return cudaSuccess;
+  if (h.n_sphere_cfgs != io->num_sphere_configs) return cudaErrorInvalidValue;
+  a.sphere_cfgs = reinterpret_cast<const float4 *>(io->sphere_configs);
+  a.n_sphere_cfgs = io->num_sphere_configs;
+  return cudaSuccess;
+}
 
 // Lower-bound pyramid level of the ESDF (see voxel_sdf_grad): one thread per block of B^3 base corners (B = kMipBlock);
 // the block of base corners [Bc, Bc+B-1] reads fine voxels [Bc, Bc+B] per axis (clipped to the grid).
@@ -2182,10 +2170,7 @@ int cb200_kinematics_forward_spheres(float *link_pos, float *link_quat, float *b
                link_masses_com, batch_center_of_mass};
   const size_t smem = (size_t)kWarpsPerCta * num_links * 12 * sizeof(float);
   void (*kern)(const KinFwdArgs) = compute_com != 0 ? kin_forward_kernel<true> : kin_forward_kernel<false>;
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return ret(e);
-  }
+  if (const cudaError_t e = opt_in_smem(kern, smem); e != cudaSuccess) return e;
   const int grid = persistent_grid(kern, kWarpsPerCta * 32, smem, (batch_size + kWarpsPerCta - 1) / kWarpsPerCta);
   CB200_LAUNCH(kern, grid, kWarpsPerCta * 32, smem, (cudaStream_t)stream, a);
   return launch_status();
@@ -2221,10 +2206,7 @@ int cb200_kinematics_backward(float *grad_out, const float *grad_nlinks_pos, con
   void (*kern)(const KinBwdArgs) = compute_com != 0 ? kin_backward_kernel<true> : kin_backward_kernel<false>;
   const size_t per_warp = ((size_t)num_links * 12 + num_links * 8 + num_links + n_joints + 3) & ~(size_t)3;
   const size_t smem = ((((size_t)2 * num_links + 3) & ~(size_t)3) + kWarpsPerCta * per_warp) * sizeof(float);
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return ret(e);
-  }
+  if (const cudaError_t e = opt_in_smem(kern, smem); e != cudaSuccess) return e;
   const int grid = persistent_grid(kern, kWarpsPerCta * 32, smem, (batch_size + kWarpsPerCta - 1) / kWarpsPerCta);
   CB200_LAUNCH(kern, grid, kWarpsPerCta * 32, smem, (cudaStream_t)stream, a);
   return launch_status();
@@ -2247,11 +2229,9 @@ int cb200_self_collision_distance(float *out_distance, float *out_vec, float *pa
   SelfArgs a{out_distance, out_vec, pair_distance, sparse_index, robot_spheres, sphere_padding, weight,
              reinterpret_cast<const uint32_t *>(pair_locations), N, nspheres, num_collision_pairs, store_pair_distance,
              compute_grad};
-  cudaError_t e = cudaSuccess;
   if (num_collision_pairs <= 4096) {
     const size_t smem = (size_t)8 * nspheres * 16;
-    if (smem > 48 * 1024) e = cudaFuncSetAttribute(self_collision_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return ret(e);
+    if (const cudaError_t e = opt_in_smem(self_collision_kernel<32>, smem); e != cudaSuccess) return e;
     const int grid = persistent_grid(self_collision_kernel<32>, 256, smem, (N + 7) / 8);
     CB200_LAUNCH(self_collision_kernel<32>, grid, 256, smem, (cudaStream_t)stream, a);
   } else {
@@ -2301,12 +2281,9 @@ int cb200_sphere_mesh_collision(float *distance, float *gradient, const float *s
   CB200_DEVICE_GUARD(distance);
   const long long total = (long long)batch_size * horizon * num_spheres;
   if (total == 0) return ret(cudaSuccess);
-  if (total < 0 || meshes == nullptr || meshes->nodes == nullptr || meshes->triangles == nullptr ||
-      (enable_speed_metric && speed_dt == nullptr))
+  MeshSet ms;
+  if (total < 0 || meshes == nullptr || to_dev(meshes, ms) != cudaSuccess || (enable_speed_metric && speed_dt == nullptr))
     return ret(cudaErrorInvalidValue);
-  MeshSet ms{reinterpret_cast<const float4 *>(meshes->nodes), reinterpret_cast<const float4 *>(meshes->triangles),
-             meshes->node_offset, meshes->triangle_offset, meshes->dims, meshes->inv_pose, meshes->enable, meshes->count,
-             meshes->max_n, meshes->num_envs};
   MeshSceneArgs a{distance, gradient, spheres, weight, activation_distance, speed_dt, ms, env_query_idx, batch_size, horizon,
                   num_spheres, use_multi_env && env_query_idx != nullptr, sweep, enable_speed_metric, accumulate};
   const int grid = persistent_grid(mesh_collision_kernel, 128, 0, (total + 127) / 128);
@@ -2637,12 +2614,9 @@ int64_t cb200_pack_robot_blob(void *out, int64_t out_bytes, const cb200_robot_si
 int cb200_refresh_robot_spheres(void *robot_blob, const void *robot_blob_host, int32_t robot_blob_bytes, const float *link_spheres,
                                 int32_t num_sphere_configs, cb200_stream_t stream) {
   CB200_DEVICE_GUARD(robot_blob);
-  if (robot_blob == nullptr || robot_blob_host == nullptr || link_spheres == nullptr ||
-      robot_blob_bytes < (int32_t)sizeof(BlobHeader))
-    return ret(cudaErrorInvalidValue);
   BlobHeader h;
-  memcpy(&h, robot_blob_host, sizeof(BlobHeader));
-  if (h.magic != kBlobMagic || h.total_bytes != robot_blob_bytes || num_sphere_configs != h.n_sphere_cfgs)
+  if (robot_blob == nullptr || link_spheres == nullptr || !read_blob_header(robot_blob_host, robot_blob_bytes, h) ||
+      num_sphere_configs != h.n_sphere_cfgs)
     return ret(cudaErrorInvalidValue);
   if (h.S == 0) return ret(cudaSuccess);
   const SphereRefreshArgs a{static_cast<unsigned char *>(robot_blob), link_spheres, h.S, h.n_sphere_cfgs, h.n_cl, h.off_spheres,
@@ -2829,9 +2803,7 @@ static int prepare_rollout(const cb200_rollout_cfg *cfg, const cb200_rollout_io 
   r.H = io->horizon;
   r.N = (long long)io->batch_size * io->horizon;
   if (r.N == 0) return ret(cudaSuccess);
-  if (io->robot_blob_host == nullptr) return ret(cudaErrorInvalidValue);
-  memcpy(&r.h, io->robot_blob_host, sizeof(BlobHeader));
-  if (r.h.magic != kBlobMagic || r.h.total_bytes != io->robot_blob_bytes) return ret(cudaErrorInvalidValue);
+  if (!read_blob_header(io->robot_blob_host, io->robot_blob_bytes, r.h)) return ret(cudaErrorInvalidValue);
   const BlobHeader &h = r.h;
   a.cfg = *cfg;
   a.q = io->q;
@@ -2882,12 +2854,7 @@ static int prepare_rollout(const cb200_rollout_cfg *cfg, const cb200_rollout_io 
       a.cur_dt = io->current_state_dt;
     }
   }
-  if (io->sphere_configs != nullptr && io->num_sphere_configs > 1) {
-    // the broad-phase bounds in the blob must cover every configuration
-    if (h.n_sphere_cfgs != io->num_sphere_configs) return ret(cudaErrorInvalidValue);
-    a.sphere_cfgs = reinterpret_cast<const float4 *>(io->sphere_configs);
-    a.n_sphere_cfgs = io->num_sphere_configs;
-  }
+  if (set_sphere_cfgs(io, h, a) != cudaSuccess) return ret(cudaErrorInvalidValue);
   a.blob_smem_bytes = h.smem_bytes;
   r.grad_floats = eval_smem_floats(h.nl, h.D, h.S, h.L, h.n_cl);
   r.cost_floats = cost_smem_floats(h.nl, h.D, h.S, h.n_cl, h.n_lp == 0);
@@ -2895,15 +2862,9 @@ static int prepare_rollout(const cb200_rollout_cfg *cfg, const cb200_rollout_io 
                       sp->out_acceleration != nullptr && sp->out_jerk != nullptr && sp->out_dt != nullptr;
   // mesh obstacles: scene bit 2.  The in-kernel spline schedule and the fused-dynamics kernel have no mesh build; they refuse mesh
   // scenes rather than drop the meshes (the expanded schedule and the host-composed dynamics cost support them).
-  r.mesh = cfg->scene_weight > 0.0f && io->meshes != nullptr && io->meshes->inv_pose != nullptr;
-  if (r.mesh) {
-    const cb200_mesh_set *m = io->meshes;
-    if (m->nodes == nullptr || m->triangles == nullptr || m->node_offset == nullptr || m->triangle_offset == nullptr ||
-        m->dims == nullptr || m->enable == nullptr || m->count == nullptr || (sp != nullptr && !expand) || io->dynamics != nullptr)
-      return ret(cudaErrorInvalidValue);
-    a.meshes = MeshSet{reinterpret_cast<const float4 *>(m->nodes), reinterpret_cast<const float4 *>(m->triangles), m->node_offset,
-                       m->triangle_offset, m->dims, m->inv_pose, m->enable, m->count, m->max_n, m->num_envs};
-  }
+  if (cfg->scene_weight > 0.0f && to_dev(io->meshes, a.meshes) != cudaSuccess) return ret(cudaErrorInvalidValue);
+  r.mesh = a.meshes.inv_pose != nullptr;
+  if (r.mesh && ((sp != nullptr && !expand) || io->dynamics != nullptr)) return ret(cudaErrorInvalidValue);
   if (expand) {
     // expanded schedule: knots -> state with the stand-alone spline kernel, then the plain rollout kernels read it
     const int rc = cb200_bspline_forward(sp->out_position, sp->out_velocity, sp->out_acceleration, sp->out_jerk, sp->out_dt,
@@ -3007,10 +2968,8 @@ int cb200_rollout_validate(const cb200_rollout_io *io, uint8_t *valid, int32_t c
     return ret(cudaErrorInvalidValue);
   const long long N = (long long)io->batch_size * io->horizon;
   if (N == 0) return ret(cudaSuccess);
-  if (io->robot_blob_host == nullptr || N > 0x7fffffffLL) return ret(cudaErrorInvalidValue);
   BlobHeader h;
-  memcpy(&h, io->robot_blob_host, sizeof(BlobHeader));
-  if (h.magic != kBlobMagic || h.total_bytes != io->robot_blob_bytes) return ret(cudaErrorInvalidValue);
+  if (N > 0x7fffffffLL || !read_blob_header(io->robot_blob_host, io->robot_blob_bytes, h)) return ret(cudaErrorInvalidValue);
   FusedArgs a{};
   a.cfg.self_weight = 1.0f;
   a.cfg.scene_weight = 1.0f;
@@ -3022,25 +2981,13 @@ int cb200_rollout_validate(const cb200_rollout_io *io, uint8_t *valid, int32_t c
   a.H = io->horizon;
   a.blob_smem_bytes = h.smem_bytes;
   a.eval_floats = cost_smem_floats(h.nl, h.D, h.S, h.n_cl, h.n_lp == 0);
-  if (io->sphere_configs != nullptr && io->num_sphere_configs > 1) {
-    if (h.n_sphere_cfgs != io->num_sphere_configs) return ret(cudaErrorInvalidValue);
-    a.sphere_cfgs = reinterpret_cast<const float4 *>(io->sphere_configs);
-    a.n_sphere_cfgs = io->num_sphere_configs;
-  }
+  if (set_sphere_cfgs(io, h, a) != cudaSuccess) return ret(cudaErrorInvalidValue);
   int scene = 0;
   if (check_scene) {
     a.cuboids = to_dev(io->cuboids);
     a.voxels = to_dev(io->voxels);
-    scene = (a.cuboids.inv_pose ? 1 : 0) | (a.voxels.inv_pose ? 2 : 0);
-    const cb200_mesh_set *m = io->meshes;
-    if (m != nullptr && m->inv_pose != nullptr) {
-      if (m->nodes == nullptr || m->triangles == nullptr || m->node_offset == nullptr || m->triangle_offset == nullptr ||
-          m->dims == nullptr || m->enable == nullptr || m->count == nullptr)
-        return ret(cudaErrorInvalidValue);
-      a.meshes = MeshSet{reinterpret_cast<const float4 *>(m->nodes), reinterpret_cast<const float4 *>(m->triangles), m->node_offset,
-                         m->triangle_offset, m->dims, m->inv_pose, m->enable, m->count, m->max_n, m->num_envs};
-      scene = 7;
-    }
+    if (to_dev(io->meshes, a.meshes) != cudaSuccess) return ret(cudaErrorInvalidValue);
+    scene = a.meshes.inv_pose ? 7 : (a.cuboids.inv_pose ? 1 : 0) | (a.voxels.inv_pose ? 2 : 0);
   }
   const void *kernel = by_scene<true>(scene, [](auto c) { return rollout_validate_kernel<c>; });
   const DevInfo &d = dev_info();

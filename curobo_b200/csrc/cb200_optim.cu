@@ -27,19 +27,12 @@
 #include "cb200_launch.h"
 
 namespace {
+using cb200::launch_status;
+using cb200::opt_in_smem;
+using cb200::persistent_grid;
+using cb200::ret;
 
 constexpr unsigned kFull = 0xffffffffu;
-
-inline int status(cudaError_t e) {
-  if (e != cudaSuccess) (void)cudaGetLastError();
-  return (int)e;
-}
-
-int sm_count() {
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms;
-}
 
 // ---- reductions ----------------------------------------------------------------------------------------------------
 // Shuffle-down tree over a group of G lanes (absent elements hold 0, which the reference's masked tree skips:
@@ -421,28 +414,16 @@ __global__ void line_search_block_kernel(const __grid_constant__ LineSearchArgs 
   }
 }
 
-template <class K>
-int persistent_grid(K kern, int block, size_t smem, long long work) {
-  int per_sm = 1;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, block, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-  long long g = (long long)sm_count() * per_sm;
-  if (g > work) g = work;
-  return (int)(g < 1 ? 1 : g);
-}
-
 template <int G>
 int launch_lbfgs_group(const LbfgsArgs &a, cudaStream_t stream) {
   constexpr int P = 32 / G;
   const int block = 128, nwarps = block / 32;
   const size_t smem = (size_t)nwarps * (2 * a.m * 32 + 2 * P * 32) * sizeof(float);
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(lbfgs_step_group_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return status(e);
-  }
+  if (const cudaError_t e = opt_in_smem(lbfgs_step_group_kernel<G>, smem); e != cudaSuccess) return e;
   const long long groups = ((long long)a.B + P - 1) / P;
   const int grid = persistent_grid(lbfgs_step_group_kernel<G>, block, smem, (groups + nwarps - 1) / nwarps);
   CB200_LAUNCH(lbfgs_step_group_kernel<G>, grid, block, smem, stream, a);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 template <int G>
 int launch_ls_group(const LineSearchArgs &a, cudaStream_t stream) {
@@ -451,7 +432,7 @@ int launch_ls_group(const LineSearchArgs &a, cudaStream_t stream) {
   const long long groups = ((long long)a.B + P - 1) / P;
   const int grid = persistent_grid(line_search_group_kernel<G>, block, 0, (groups + nwarps - 1) / nwarps);
   CB200_LAUNCH(line_search_group_kernel<G>, grid, block, 0, stream, a);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 // ---- MPPI sample -----------------------------------------------------------------------------------------------------
@@ -650,7 +631,7 @@ int launch_mppi_group(const MppiUpdateArgs &a, cudaStream_t stream) {
   constexpr int NG = 128 / G;
   const size_t smem = (size_t)NG * (a.Np + a.H * a.D) * sizeof(float);
   CB200_LAUNCH(mppi_update_group_kernel<G>, (a.P + NG - 1) / NG, 128, smem, stream, a);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 }  // namespace
 
@@ -665,10 +646,10 @@ int cb200_lbfgs_step(float *step_vec, float *rho_buffer, float *y_buffer, float 
   if (step_vec == nullptr || rho_buffer == nullptr || y_buffer == nullptr || s_buffer == nullptr || q == nullptr ||
       grad_q == nullptr || x_0 == nullptr || grad_0 == nullptr || batch_size < 0 || v_dim < 1 || v_dim > 1024 ||
       history_m < 1 || history_m > 31)
-    return status(cudaErrorInvalidValue);
+    return ret(cudaErrorInvalidValue);
   if (x_set != nullptr && (search_magnitudes == nullptr || n_linesearch < 1 || (action_step_max != nullptr && action_dim < 1)))
-    return status(cudaErrorInvalidValue);
-  if (batch_size == 0) return status(cudaSuccess);
+    return ret(cudaErrorInvalidValue);
+  if (batch_size == 0) return ret(cudaSuccess);
   LbfgsArgs a{step_vec, rho_buffer, y_buffer, s_buffer, x_0, grad_0, q, grad_q, epsilon, batch_size, history_m, v_dim,
               stable_mode, x_set, step_scaled, search_magnitudes, action_step_max, n_linesearch, action_dim < 1 ? 1 : action_dim,
               (fix_terminal_action && action_dim > 0 && v_dim > action_dim) ? v_dim - action_dim : v_dim};
@@ -679,7 +660,7 @@ int cb200_lbfgs_step(float *step_vec, float *rho_buffer, float *y_buffer, float 
   if (v_dim <= 32) return launch_lbfgs_group<32>(a, st);
   const int block = (v_dim + 31) / 32 * 32;
   CB200_LAUNCH(lbfgs_step_block_kernel, batch_size, block, 2 * history_m * sizeof(float), st, a);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 int cb200_line_search(float *best_cost, float *best_action, int16_t *best_iteration, int16_t *current_iteration,
@@ -699,8 +680,8 @@ int cb200_line_search(float *best_cost, float *best_action, int16_t *best_iterat
       search_action == nullptr || search_gradient == nullptr || step_direction == nullptr ||
       search_magnitudes == nullptr || n_linesearch < 1 || n_linesearch > 32 || opt_dim < 1 || opt_dim > 1024 ||
       batchsize < 0)
-    return status(cudaErrorInvalidValue);
-  if (batchsize == 0) return status(cudaSuccess);
+    return ret(cudaErrorInvalidValue);
+  if (batchsize == 0) return ret(cudaSuccess);
   LineSearchArgs a{best_cost, best_action, best_iteration, current_iteration, converged_global, convergence_iteration,
                    cost_delta_threshold, cost_relative_threshold, exploration_cost, exploration_action,
                    exploration_gradient, exploration_idx, selected_cost, selected_action, selected_gradient, selected_idx,
@@ -713,7 +694,7 @@ int cb200_line_search(float *best_cost, float *best_action, int16_t *best_iterat
   if (opt_dim <= 32) return launch_ls_group<32>(a, st);
   const int block = (opt_dim + 31) / 32 * 32;
   CB200_LAUNCH(line_search_block_kernel, batchsize, block, 0, st, a);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 int cb200_mppi_sample(float *actions, const float *mean, const float *scale, const float *noise, const float *lows,
@@ -724,13 +705,13 @@ int cb200_mppi_sample(float *actions, const float *mean, const float *scale, con
       num_problems < 0 || num_particles < 1 || num_sampled < 1 || num_neg < 0 || num_sampled + num_neg > num_particles ||
       horizon < 1 || action_dim < 1 ||
       (long long)num_problems * num_particles * horizon * action_dim > 0x7fffffffLL)
-    return status(cudaErrorInvalidValue);
-  if (num_problems == 0) return status(cudaSuccess);
+    return ret(cudaErrorInvalidValue);
+  if (num_problems == 0) return ret(cudaSuccess);
   const int HD = horizon * action_dim, total = num_problems * num_particles * HD;
   MppiSampleArgs a{actions, mean, scale, noise, lows, highs, total, num_particles, num_sampled, num_neg, HD, action_dim,
                    noise_per_problem ? num_sampled * HD : 0};
   CB200_LAUNCH(mppi_sample_kernel, (total + 255) / 256, 256, 0, (cudaStream_t)stream, a);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 int cb200_mppi_update(const float *actions, const float *cost, float *mean, float *cov, float *scale, float *best,
@@ -741,8 +722,8 @@ int cb200_mppi_update(const float *actions, const float *cost, float *mean, floa
   if (actions == nullptr || cost == nullptr || mean == nullptr || (update_cov && (cov == nullptr || scale == nullptr)) ||
       (best_mode && best == nullptr) || num_problems < 0 || num_particles < 1 || horizon < 1 || action_dim < 1 ||
       !(beta > 0.0f) || num_particles + V > kMppiMaxSmemFloats)
-    return status(cudaErrorInvalidValue);
-  if (num_problems == 0) return status(cudaSuccess);
+    return ret(cudaErrorInvalidValue);
+  if (num_problems == 0) return ret(cudaSuccess);
   // the coefficients as torch forms them: Python-double scalars rounded once to float
   MppiUpdateArgs a{actions, cost, mean, cov, scale, best, num_problems, num_particles, horizon, action_dim,
                    (float)(-1.0 / (double)beta), discount, step_size_mean, (float)(1.0 - (double)step_size_mean),
@@ -754,7 +735,7 @@ int cb200_mppi_update(const float *actions, const float *cost, float *mean, floa
     return launch_mppi_group<32>(a, st);
   }
   CB200_LAUNCH(mppi_update_block_kernel, num_problems, kMppiBlock, (num_particles + V) * sizeof(float), st, a);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 }  // extern "C"

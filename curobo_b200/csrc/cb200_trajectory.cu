@@ -17,11 +17,9 @@
 
 namespace {
 using namespace cb200::bspline;
-
-inline int status(cudaError_t e) {
-  if (e != cudaSuccess) (void)cudaGetLastError();  // never leave a sticky error behind for the caller's next CUDA call
-  return (int)e;
-}
+using cb200::capped_grid;
+using cb200::launch_status;
+using cb200::ret;
 
 struct FwdArgs {
   float *out_p, *out_v, *out_a, *out_j, *out_dt;
@@ -94,27 +92,17 @@ __global__ void __launch_bounds__(256) bspline_backward_kernel(const __grid_cons
   }
 }
 
-int grid_for(long long n, int block) {
-  long long g = (n + block - 1) / block;
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const long long cap = (long long)sms * 8;  // 8 x 256 threads / SM resident: a whole number of waves
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-
 int launch_forward(const FwdArgs &a, int degree, cudaStream_t stream) {
-  if (a.B <= 0 || a.T <= 0 || a.D <= 0 || a.n_knots <= 0) return status(cudaErrorInvalidValue);
+  if (a.B <= 0 || a.T <= 0 || a.D <= 0 || a.n_knots <= 0) return ret(cudaErrorInvalidValue);
   const long long n = (long long)a.B * a.T * a.D;
-  const int grid = grid_for(n, 256);
+  const int grid = capped_grid((n + 255) / 256, 8);  // 8 x 256 threads / SM resident: a whole number of waves
   switch (degree) {
     case 3: CB200_LAUNCH(bspline_forward_kernel<3>, grid, 256, 0, stream, a); break;
     case 4: CB200_LAUNCH(bspline_forward_kernel<4>, grid, 256, 0, stream, a); break;
     case 5: CB200_LAUNCH(bspline_forward_kernel<5>, grid, 256, 0, stream, a); break;
-    default: return status(cudaErrorInvalidValue);
+    default: return ret(cudaErrorInvalidValue);
   }
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -310,7 +298,7 @@ int cb200_bspline_single_dt(float *out_position, float *out_velocity, float *out
                             int bspline_degree, cb200_stream_t stream) {
   CB200_DEVICE_GUARD(out_position);
   (void)knot_dt;  // carried by the reference signature, never read by its kernel (bspline_kernel.cuh:216-270)
-  if (interpolation_horizon == nullptr) return status(cudaErrorInvalidValue);
+  if (interpolation_horizon == nullptr) return ret(cudaErrorInvalidValue);
   FwdArgs a{out_position, out_velocity, out_acceleration, out_jerk, out_dt, u_position, start_position, start_velocity,
             start_acceleration, start_jerk, goal_position, goal_velocity, goal_acceleration, goal_jerk, start_idx, goal_idx,
             interpolation_dt, use_implicit_goal_state, interpolation_horizon, batch_size, max_out_tsteps, dof, n_knots};
@@ -324,20 +312,20 @@ int cb200_bspline_backward(float *out_grad_knots, const float *grad_position, co
   CB200_DEVICE_GUARD(out_grad_knots);
   const int horizon = padded_horizon - 1;
   // same argument checks as the reference launcher (trajectory_kernel_launch.cu:592-627)
-  if (batch_size <= 0 || dof <= 0 || n_knots <= 0 || horizon < 5) return status(cudaErrorInvalidValue);
-  if (bspline_degree < 3 || bspline_degree > 5) return status(cudaErrorInvalidValue);
+  if (batch_size <= 0 || dof <= 0 || n_knots <= 0 || horizon < 5) return ret(cudaErrorInvalidValue);
+  if (bspline_degree < 3 || bspline_degree > 5) return ret(cudaErrorInvalidValue);
   const int steps = horizon / (n_knots + bspline_degree + 1);
-  if (steps <= 0 || steps > 32) return status(cudaErrorInvalidValue);
+  if (steps <= 0 || steps > 32) return ret(cudaErrorInvalidValue);
   BwdArgs a{out_grad_knots, grad_position, grad_velocity, grad_acceleration, grad_jerk, traj_dt, dt_idx, use_implicit_goal_state,
             batch_size, padded_horizon, dof, n_knots};
   const long long n = (long long)batch_size * n_knots * dof;
-  const int grid = grid_for(n, 128);
+  const int grid = capped_grid((n + 127) / 128, 8);
   switch (bspline_degree) {
     case 3: CB200_LAUNCH(bspline_backward_kernel<3>, grid, 128, 0, (cudaStream_t)stream, a); break;
     case 4: CB200_LAUNCH(bspline_backward_kernel<4>, grid, 128, 0, (cudaStream_t)stream, a); break;
     default: CB200_LAUNCH(bspline_backward_kernel<5>, grid, 128, 0, (cudaStream_t)stream, a); break;
   }
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 int cb200_position_clique_forward(float *out_position, float *out_velocity, float *out_acceleration, float *out_jerk,
@@ -351,13 +339,13 @@ int cb200_position_clique_forward(float *out_position, float *out_velocity, floa
   (void)goal_acceleration;
   if (batch_size == 0) return 0;
   // horizon >= 8: the reference's rows 1..3 read actions 1..3 for any horizon (past the row's actions below 8)
-  if (batch_size < 0 || dof <= 0 || horizon < 8) return status(cudaErrorInvalidValue);
+  if (batch_size < 0 || dof <= 0 || horizon < 8) return ret(cudaErrorInvalidValue);
   CliqueFwdArgs a{out_position, out_velocity, out_acceleration, out_jerk, out_dt, u_position, start_position, start_velocity,
                   start_acceleration, goal_position, start_idx, goal_idx, traj_dt, use_implicit_goal_state, batch_size,
                   horizon, dof};
-  const int grid = grid_for((long long)batch_size * horizon * dof, 256);
+  const int grid = capped_grid(((long long)batch_size * horizon * dof + 255) / 256, 8);
   CB200_LAUNCH(clique_forward_kernel, grid, 256, 0, (cudaStream_t)stream, a);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 int cb200_position_clique_backward(float *out_grad_position, const float *grad_position, const float *grad_velocity,
@@ -366,12 +354,12 @@ int cb200_position_clique_backward(float *out_grad_position, const float *grad_p
                                    int dof, cb200_stream_t stream) {
   CB200_DEVICE_GUARD(out_grad_position);
   if (batch_size == 0) return 0;
-  if (batch_size < 0 || dof <= 0 || horizon < 8) return status(cudaErrorInvalidValue);
+  if (batch_size < 0 || dof <= 0 || horizon < 8) return ret(cudaErrorInvalidValue);
   CliqueBwdArgs a{out_grad_position, grad_position, grad_velocity, grad_acceleration, grad_jerk, traj_dt, dt_idx,
                   use_implicit_goal_state, batch_size, horizon, dof};
-  const int grid = grid_for((long long)batch_size * (horizon - 4) * dof, 256);
+  const int grid = capped_grid(((long long)batch_size * (horizon - 4) * dof + 255) / 256, 8);
   CB200_LAUNCH(clique_backward_kernel, grid, 256, 0, (cudaStream_t)stream, a);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 int cb200_acceleration_integrate(float *out_position, float *out_velocity, float *out_acceleration, float *out_jerk,
@@ -381,12 +369,12 @@ int cb200_acceleration_integrate(float *out_position, float *out_velocity, float
   CB200_DEVICE_GUARD(out_position);
   (void)use_rk2;   // both reference kernels compute the same semi-implicit Euler step
   if (batch_size == 0) return 0;
-  if (batch_size < 0 || dof <= 0 || horizon < 1) return status(cudaErrorInvalidValue);
+  if (batch_size < 0 || dof <= 0 || horizon < 1) return ret(cudaErrorInvalidValue);
   IntegrateArgs a{out_position, out_velocity, out_acceleration, out_jerk, u_acc, start_position, start_velocity,
                   start_acceleration, start_idx, traj_dt, batch_size, horizon, dof};
-  const int grid = grid_for((long long)batch_size * dof, 128);
+  const int grid = capped_grid(((long long)batch_size * dof + 127) / 128, 8);
   CB200_LAUNCH(acceleration_integrate_kernel, grid, 128, 0, (cudaStream_t)stream, a);
-  return status(cudaGetLastError());
+  return launch_status();
 }
 
 }  // extern "C"
