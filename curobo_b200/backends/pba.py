@@ -99,6 +99,36 @@ def launch_tsdf_integrate_depth(block_data: torch.Tensor, nx: int, ny: int, nz: 
     _lib.check(err, "tsdf_integrate_depth")
 
 
+
+def launch_segment_robot_depth(depth_images: torch.Tensor, intrinsics: torch.Tensor, cam_positions: torch.Tensor,
+                               cam_quaternions: torch.Tensor, robot_spheres: torch.Tensor, distance_threshold: float,
+                               mask: torch.Tensor, filtered: torch.Tensor) -> None:
+    """The robot's own pixels of depth_images [B, H, W] (float32, metres): mask (bool or uint8 [B, H, W]) = depth > 0 and the
+    pixel's point within distance_threshold of a sphere of robot_spheres [1 or B, S, 4] (robot base frame); filtered (float32
+    [B, H, W]) = depth with the masked pixels set to 0.  intrinsics [B, 3, 3], cam_positions [B, 3], cam_quaternions [B, 4]
+    (wxyz, camera -> robot base): the tensors launch_tsdf_integrate_depth takes.  RobotSegmenter._mask_op
+    (robot_segmenter.py:267-366) in one launch."""
+    dev = depth_images.device
+    check_tensors(dev, torch.float32, depth_images=depth_images, intrinsics=intrinsics, cam_positions=cam_positions,
+                  cam_quaternions=cam_quaternions, robot_spheres=robot_spheres, filtered=filtered)
+    if mask.dtype not in (torch.bool, torch.uint8):
+        raise ValueError(f"mask: expected dtype torch.bool or torch.uint8, got {mask.dtype}")
+    check_tensors(dev, mask.dtype, mask=mask)
+    if depth_images.dim() != 3:
+        raise ValueError("depth_images must be [batch, height, width]")
+    b, h, w = (int(v) for v in depth_images.shape)
+    if intrinsics.numel() != 9 * b or cam_positions.numel() != 3 * b or cam_quaternions.numel() != 4 * b:
+        raise ValueError("intrinsics / cam_positions / cam_quaternions must be [B,3,3] / [B,3] / [B,4] for B = depth_images.shape[0]")
+    if robot_spheres.dim() != 3 or robot_spheres.shape[-1] != 4 or robot_spheres.shape[0] not in (1, b):
+        raise ValueError(f"robot_spheres must be [1 or {b}, num_spheres, 4], got {tuple(robot_spheres.shape)}")
+    if tuple(mask.shape) != (b, h, w) or tuple(filtered.shape) != (b, h, w):
+        raise ValueError(f"mask / filtered must be [{b}, {h}, {w}]")
+    err = _lib.load().cb200_segment_robot_depth(depth_images.data_ptr(), b, h, w, intrinsics.data_ptr(), cam_positions.data_ptr(),
+                                                cam_quaternions.data_ptr(), robot_spheres.data_ptr(), int(robot_spheres.shape[0]),
+                                                int(robot_spheres.shape[1]), float(distance_threshold), mask.data_ptr(),
+                                                filtered.data_ptr(), stream_ptr(dev))
+    _lib.check(err, "segment_robot_depth")
+
 def launch_tsdf_combined_sdf(block_data: torch.Tensor, static_sdf, combined_sdf: torch.Tensor, min_weight: float) -> None:
     """combined_sdf (float32) = min(sum_sdf_w / sum_w where sum_w > min_weight else 1e10, static_sdf): sample_combined_sdf
     (wp_tsdf_sample.py:22-97) for the dense grid."""

@@ -258,6 +258,128 @@ __global__ void __launch_bounds__(256) tsdf_integrate_depth_kernel(__half *__res
   }
 }
 
+// Robot pixels of depth images, masked before the images reach the integrator above: the reference's RobotSegmenter
+// (perception/robot_segmenter.py:35-366, rays of geom/cv.py:47-157) without its [pixels x spheres] distance matrix.  One CTA per
+// 32 x 8 pixel tile of one image, warp = tile row (one 128-byte line of depth / filtered):
+//   1. every thread deprojects its pixel and moves it into the robot frame; a block reduction gives the box of the tile's
+//      candidate points (depth > 0 and finite),
+//   2. the CTA keeps the image's spheres whose distance to that box is under r + threshold, compacted into shared memory,
+//   3. every candidate pixel scans the kept spheres and stops at the first hit.
+// A tile without a candidate skips 2 and 3.  The cull is exact: box and pixel distances round the same way (seg_dist2), and for a
+// point inside the box every per-axis box gap is at most the point's rounded offset (rounding is monotone), so a sphere a pixel
+// hits is never culled.
+constexpr int kSegTileW = 32, kSegTileH = 8, kSegThreads = kSegTileW * kSegTileH, kSegWarps = kSegThreads / 32;
+struct SegmentArgs {
+  const float *depth;       // [B, H, W] metres
+  const float *intrinsics;  // [B, 3, 3]
+  const float *position;    // [B, 3]
+  const float *quaternion;  // [B, 4] wxyz, camera -> robot base
+  const float *spheres;     // [1 or B, S, 4]
+  uint8_t *mask;            // [B, H, W]
+  float *filtered;          // [B, H, W]
+  int height, width, tiles_x, tiles_per_image;
+  int sphere_stride;        // floats between two images' spheres: 0 when one robot state serves every image
+  int num_spheres;
+  float threshold;
+};
+// |d|^2 in round-to-nearest steps that the compiler cannot contract, so that the cull and the pixel test round alike
+__device__ __forceinline__ float seg_dist2(float dx, float dy, float dz) {
+  return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+}
+__global__ void __launch_bounds__(kSegThreads) segment_robot_depth_kernel(const SegmentArgs a) {
+  using namespace cb200;
+  CB200_EXTERN_SHARED __align__(16) float smem[];  // kept spheres: (centre, (r + threshold)^2)
+  __shared__ float warp_box[kSegWarps][7];         // lo xyz, hi xyz, any candidate
+  __shared__ int kept;
+  float4 *survivors = reinterpret_cast<float4 *>(smem);
+  const unsigned full = 0xffffffffu;
+  const float inf = __int_as_float(0x7f800000);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int img = blockIdx.x / a.tiles_per_image, tile = blockIdx.x - img * a.tiles_per_image;
+  const int tile_y = tile / a.tiles_x;
+  const int u = (tile - tile_y * a.tiles_x) * kSegTileW + lane, v = tile_y * kSegTileH + warp;
+  const bool inside = u < a.width && v < a.height;
+  const long long pix = ((long long)img * a.height + v) * a.width + u;
+  const float d = inside ? a.depth[pix] : 0.0f;
+  // the reference masks depth > 0 only; an infinite depth puts the point at infinity and NaN fails every comparison, so
+  // neither is ever masked there.  Tested on the bits: the library flushes subnormals to zero, and `d > 0.0f` would drop a
+  // subnormal positive depth that the reference can mask.
+  const int dbits = __float_as_int(d);
+  const bool cand = dbits > 0 && dbits < 0x7f800000;
+  V3 p = mk3(0.0f, 0.0f, 0.0f);
+  if (cand) {
+    const float *K = a.intrinsics + 9 * img, *cp = a.position + 3 * img, *cq = a.quaternion + 4 * img;
+    // ray ((u - cx) / fx, (v - cy) / fy, 1) times the depth (get_projection_rays, project_depth_using_rays); IEEE divisions,
+    // as in tsdf_integrate_depth_kernel
+    const V3 pc = mk3(__fmul_rn(__fdiv_rn(__fsub_rn((float)u, K[2]), K[0]), d), __fmul_rn(__fdiv_rn(__fsub_rn((float)v, K[5]), K[4]), d), d);
+    p = qrot(Q4{cq[1], cq[2], cq[3], cq[0]}, pc) + mk3(cp[0], cp[1], cp[2]);
+  }
+  float lo[3] = {cand ? p.x : inf, cand ? p.y : inf, cand ? p.z : inf};
+  float hi[3] = {cand ? p.x : -inf, cand ? p.y : -inf, cand ? p.z : -inf};
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      lo[k] = fminf(lo[k], __shfl_xor_sync(full, lo[k], off));
+      hi[k] = fmaxf(hi[k], __shfl_xor_sync(full, hi[k], off));
+    }
+  }
+  const unsigned warp_cand = __ballot_sync(full, cand);
+  if (lane == 0) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) warp_box[warp][k] = lo[k], warp_box[warp][3 + k] = hi[k];
+    warp_box[warp][6] = warp_cand ? 1.0f : 0.0f;
+  }
+  if (threadIdx.x == 0) kept = 0;
+  __syncthreads();
+  bool any = false;
+#pragma unroll
+  for (int w = 0; w < kSegWarps; ++w) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) lo[k] = fminf(lo[k], warp_box[w][k]), hi[k] = fmaxf(hi[k], warp_box[w][3 + k]);
+    any = any || warp_box[w][6] != 0.0f;
+  }
+  bool hit = false;
+  if (any) {  // the same for every thread of the CTA
+    const float *sph = a.spheres + (long long)img * a.sphere_stride;
+    for (int base = 0; base < a.num_spheres; base += kSegThreads) {
+      const int k = base + (int)threadIdx.x;
+      bool keep = false;
+      float4 s = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+      if (k < a.num_spheres) {
+        const float cx = sph[4 * k], cy = sph[4 * k + 1], cz = sph[4 * k + 2], reach = sph[4 * k + 3] + a.threshold;
+        if (reach > 0.0f) {  // a disabled sphere (radius -100) never masks
+          const float gx = fmaxf(fmaxf(__fsub_rn(lo[0], cx), __fsub_rn(cx, hi[0])), 0.0f);
+          const float gy = fmaxf(fmaxf(__fsub_rn(lo[1], cy), __fsub_rn(cy, hi[1])), 0.0f);
+          const float gz = fmaxf(fmaxf(__fsub_rn(lo[2], cz), __fsub_rn(cz, hi[2])), 0.0f);
+          s = make_float4(cx, cy, cz, __fmul_rn(reach, reach));
+          keep = seg_dist2(gx, gy, gz) < s.w;
+        }
+      }
+      const unsigned m = __ballot_sync(full, keep);
+      int slot = 0;
+      if (lane == 0 && m != 0u) slot = atomicAdd(&kept, __popc(m));
+      slot = __shfl_sync(full, slot, 0);
+      if (keep) survivors[slot + __popc(m & ((1u << lane) - 1u))] = s;
+    }
+    __syncthreads();
+    const int n = kept;
+    if (cand) {
+      for (int j = 0; j < n; ++j) {
+        const float4 s = survivors[j];
+        if (seg_dist2(__fsub_rn(p.x, s.x), __fsub_rn(p.y, s.y), __fsub_rn(p.z, s.z)) < s.w) {
+          hit = true;
+          break;
+        }
+      }
+    }
+  }
+  if (inside) {
+    a.mask[pix] = hit ? 1 : 0;
+    a.filtered[pix] = hit ? 0.0f : d;
+  }
+}
+
 // combined SDF of the dynamic (depth) and static channels: wp_tsdf_sample.py:22-97 (sample_dynamic_sdf / sample_combined_sdf):
 // sum_sdf_w / sum_w where the weight exceeds min_weight, else 1e10 (unobserved); min with the static SDF when there is one.
 __global__ void __launch_bounds__(256) tsdf_combined_sdf_kernel(const __half *__restrict__ block_data, const float *__restrict__ static_sdf,
@@ -397,6 +519,29 @@ int cb200_tsdf_integrate_depth(uint16_t *block_data_fp16, int nx, int ny, int nz
   CB200_LAUNCH(tsdf_integrate_depth_kernel, capped_grid((total + 255) / 256, 32), 256, 0, (cudaStream_t)stream,
                reinterpret_cast<__half *>(block_data_fp16), nx, ny, nz, total, voxel_size, origin[0], origin[1], origin[2], cams,
                depth_min, depth_max, truncation_distance);
+  return launch_status();
+}
+
+int cb200_segment_robot_depth(const float *depth, int batch, int height, int width, const float *intrinsics,
+                              const float *cam_positions, const float *cam_quaternions, const float *robot_spheres, int robot_batch,
+                              int num_spheres, float distance_threshold, uint8_t *mask, float *filtered, cb200_stream_t stream) {
+  CB200_DEVICE_GUARD(filtered);
+  if (depth == nullptr || intrinsics == nullptr || cam_positions == nullptr || cam_quaternions == nullptr ||
+      robot_spheres == nullptr || mask == nullptr || filtered == nullptr || batch < 1 || height < 1 || width < 1 ||
+      num_spheres < 0 || (robot_batch != 1 && robot_batch != batch))
+    return ret(cudaErrorInvalidValue);
+  const int tiles_x = (width + kSegTileW - 1) / kSegTileW;
+  const long long tiles_per_image = (long long)tiles_x * ((height + kSegTileH - 1) / kSegTileH);
+  // one flat grid (the host emulation of tests/simt launches along x only): its x extent bounds the batch
+  if (tiles_per_image * batch > 2147483647LL) return ret(cudaErrorInvalidValue);
+  const long long smem = (long long)num_spheres * (long long)sizeof(float4);
+  cudaFuncAttributes fa;
+  if (cudaFuncGetAttributes(&fa, segment_robot_depth_kernel) != cudaSuccess) return ret(cudaErrorInvalidConfiguration);
+  if (smem + (long long)fa.sharedSizeBytes > (long long)cb200::dev_info().max_smem) return ret(cudaErrorInvalidValue);
+  if (opt_in_smem(segment_robot_depth_kernel, (size_t)smem) != cudaSuccess) return ret(cudaErrorInvalidConfiguration);
+  const SegmentArgs a{depth, intrinsics, cam_positions, cam_quaternions, robot_spheres, mask, filtered, height, width, tiles_x,
+                      (int)tiles_per_image, robot_batch == 1 ? 0 : 4 * num_spheres, num_spheres, distance_threshold};
+  CB200_LAUNCH(segment_robot_depth_kernel, tiles_per_image * batch, kSegThreads, (size_t)smem, (cudaStream_t)stream, a);
   return launch_status();
 }
 

@@ -116,6 +116,7 @@ _SIGS = {
     "cb200_tsdf_integrate_depth": ([c_p, _I, _I, _I, C.c_float, C.POINTER(C.c_float), _I, c_p, c_p, c_p, c_p, _I, _I, C.c_float,
                                     C.c_float, C.c_float, c_p], _I),
     "cb200_tsdf_combined_sdf": ([c_p, c_p, c_p, C.c_longlong, C.c_float, c_p], _I),
+    "cb200_segment_robot_depth": ([c_p, _I, _I, _I, c_p, c_p, c_p, c_p, _I, _I, C.c_float, c_p, c_p, c_p], _I),
     "cb200_tsdf_stamp_cuboids": ([c_p, _I, _I, _I, C.c_float, C.POINTER(C.c_float), C.c_float, C.POINTER(CuboidSet), _I, c_p], _I),
     "cb200_robot_blob_bytes": ([C.POINTER(RobotSizes)], C.c_int64),
     "cb200_pack_robot_blob": ([c_p, C.c_int64, C.POINTER(RobotSizes)] + [c_p] * 15, C.c_int64),

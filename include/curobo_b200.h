@@ -626,6 +626,26 @@ int cb200_tsdf_integrate_depth(uint16_t *block_data_fp16, int nx, int ny, int nz
                                cb200_stream_t stream);
 int cb200_tsdf_combined_sdf(const uint16_t *block_data_fp16, const float *static_sdf, float *combined_sdf, long long num_voxels,
                             float min_weight, cb200_stream_t stream);
+/* Robot pixels of depth images, masked in front of cb200_tsdf_integrate_depth (same camera model, quaternion convention and
+ * depth layout):
+ *   cb200_segment_robot_depth   <- RobotSegmenter._mask_op  perception/robot_segmenter.py:267-366 with get_projection_rays /
+ *                                  project_depth_using_rays  geom/cv.py:47-157 and _mask_spheres_image_cdist.  Pixel (u, v) at
+ *                                  integer coordinates: p_cam = ((u - cx) / fx d, (v - cy) / fy d, d) (IEEE divisions),
+ *                                  p = R(q) p_cam + t.  mask = d > 0 and |p - c_s| < r_s + distance_threshold for some sphere s
+ *                                  (the reference's max_s(r_s - |p - c_s|) > -distance_threshold); a sphere with
+ *                                  r_s + distance_threshold <= 0 (a disabled sphere at radius -100) never masks, nor does a pixel
+ *                                  with non-finite depth.  d > 0 is decided on the bits, so a subnormal positive depth counts
+ *                                  although the library flushes subnormals to zero (its point is then the camera position).
+ *                                  filtered = mask ? 0 : depth, every other pixel copied bit for bit.
+ *                                  robot_spheres [robot_batch, S, 4], robot_batch 1 (one state for every image) or B.  Refused
+ *                                  (nothing launched): a NULL pointer, robot_batch neither 1 nor B, S spheres beyond the shared-
+ *                                  memory opt-in (16 bytes each), more than 2^31 - 1 tiles of 32 x 8 pixels in all. */
+int cb200_segment_robot_depth(const float *depth /* [B,H,W] metres */, int batch, int height, int width,
+                              const float *intrinsics /* [B,3,3] */, const float *cam_positions /* [B,3] */,
+                              const float *cam_quaternions /* [B,4] wxyz, camera -> robot base */,
+                              const float *robot_spheres /* [Bs,S,4], Bs == 1 or B */, int robot_batch, int num_spheres,
+                              float distance_threshold, uint8_t *mask /* [B,H,W] */, float *filtered /* [B,H,W] */,
+                              cb200_stream_t stream);
 /*   cb200_tsdf_stamp_cuboids   <- stamp_sdf_kernel  kernel/builder/builder_stamp.py:263-315 with the cuboid overloads of
  *                                  geom/data/data_cuboid.py:461-545 (the per-voxel step of BlockSparseTSDFIntegrator's obstacle
  *                                  stamping; block enumeration / allocation out of scope): static_sdf (f32, > 1e9 = nothing
